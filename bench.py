@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- the BASELINE.json workloads of the B200 OnnxStream engine, one JSON line per run.
+"""bench.py -- the BASELINE.json workloads of the OnnxStream engine on one H100, one JSON line per run.
 
-Default workload (what the driver runs): SD 1.5 UNet 512x512 bs=1 denoise-step throughput (BASELINE config[1] hot path).
+Default workload: SD 1.5 UNet 512x512 bs=1 denoise-step throughput (BASELINE config[1] hot path).
 One "step" = one UNet Model::run() on one 4x64x64 latent (the reference runs two per sampler step with CFG; the metric counts
 UNet runs).  fp16 weights / fp16 arithmetic / attention fusion, i.e. what sd.cpp sets (src/sd.cpp:1616-1683).  Synthetic
 graphs of the named architectures + seeded random weights (no checkpoints offline).
@@ -11,7 +11,7 @@ graphs of the named architectures + seeded random weights (no checkpoints offlin
   e2e     : the same metric through the reference-facing C ABI with HOST buffers: every step pushes the inputs from pinned host
             memory, streams ALL weights pinned-host -> HBM ring (the CUDA WeightsProvider; N>1: every rank uploads 1/N of each
             node over its own PCIe link and an NCCL all-gather over NVLink completes the ring slot) and reads the output back
-  roofline: the dominant kernel (tcgen05 implicit-GEMM conv / GEMM) timed per launch with CUDA events in an eager pass
+  roofline: the dominant kernel (wgmma implicit-GEMM conv / GEMM) timed per launch with CUDA events in an eager pass
   cpu_baseline / --impl reference: the reference's own CPU path (oracle/_ref: unmodified reference sources + XNNPACK), FULL
             graph runs on the host cores (no prefix extrapolation for the default workload)
   parity  : every rank checks its streamed output against its resident-weights output, and one common sample against the
@@ -20,6 +20,12 @@ graphs of the named architectures + seeded random weights (no checkpoints offlin
 Other workloads (`--workload`): sdxl_unet_w8 (SDXL 1024x1024, uint8 weights; N=2 = the CFG cond/uncond pair), sdxl_turbo_w8
 (512x512, one sample per GPU), vae_decoder_fp16, clip_text_fp32, sd15_pipeline (text encoder + 20 CFG steps + VAE decoder),
 tinyllama_decode (seq 2048).  `--all-configs FILE` runs them all and writes one line each.
+
+`--dump-outputs DIR` (by convention bench_dumps/<build>, git-ignored) writes, after the timed steps, every output a caller of the timed
+path receives as DIR/<workload>.<output>.npy in float32, so two builds can be compared output for output.  The arrays come from one
+more replay of the timed CUDA graph on the same seeded inputs (the timed replays keep their outputs on the device); above 64 MB in all,
+every array keeps the same fixed seeded fraction of its flattened values.  (The decode workloads keep the KV cache in HBM, so their
+caller receives the logits only.)
 """
 import argparse
 import ctypes
@@ -60,8 +66,8 @@ from onnxstream_b200.model import Model, ENGINE_LIB  # noqa: E402
 
 ORACLE_LIB = os.path.join(ROOT, "oracle", "_ref", "liboracle_ref.so")
 HOST_CORES = os.cpu_count() or 1
-# XNNPACK's pthreadpool with one worker per core is far slower than a moderate pool on many-core hosts (measured r01: 128
-# workers -> 295 s per UNet run on the GPU box, vs 38 s with 8 on an 8-core host), so the reference gets min(cores, 32).
+# XNNPACK's pthreadpool with one worker per core is far slower than a moderate pool on many-core hosts, so the reference gets
+# min(cores, 32).
 REF_THREADS = min(HOST_CORES, 32)
 # torchrun exports OMP_NUM_THREADS=1 to every rank: ASSIGN (the oracle's shim loops are OpenMP; the engine does not use OpenMP)
 os.environ["OMP_NUM_THREADS"] = str(REF_THREADS)
@@ -118,7 +124,7 @@ class SD15UNet(Workload):
 
 
 class SD15UNetFP32(SD15UNet):
-    """BASELINE config[0]: the SD 1.5 UNet step in fp32 (fp32 blobs, fp32 arithmetic -- the reference's default CPU mode).  On the B200 engine
+    """BASELINE config[0]: the SD 1.5 UNet step in fp32 (fp32 blobs, fp32 arithmetic -- the reference's default CPU mode).  On the engine
     every Conv / MatMul / Gemm runs on the tensor cores through the bf16 triple split (fp32-faithful); the reference arm is the same graph and
     blobs through XNNPACK f32."""
     name = "sd15_unet_fp32"
@@ -274,11 +280,8 @@ WORKLOADS = ["sd15_unet_fp16", "sd15_unet_fp32", "tiny_unet_fp16", "sdxl_unet_w8
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1450.4), d.get("hbm_gbs", 6567.7), "measured (MEASURED_PEAKS.json, sustained bf16 cuBLAS)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    # NVIDIA's H100 SXM data sheet (dense fp16 / bf16, HBM3; a card allowed 700 W): ceilings, not rates this card was seen to reach
+    return 989.0, 3350.0, "H100 SXM data sheet"
 
 
 def model_dir(workload: str) -> str:
@@ -301,7 +304,7 @@ def ensure_model(w: Workload):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self):
         self.rows = []
@@ -340,7 +343,7 @@ def dist_setup():
     import torch.distributed as dist
     torch.cuda.set_device(0)
     import datetime
-    # a rank that dies or skips a collective must not hold the others (and the GPU box) for NCCL's default 10 minutes
+    # a rank that dies or skips a collective must not hold the others (and the GPUs) for NCCL's default 10 minutes
     dist.init_process_group("nccl", device_id=torch.device("cuda", 0), timeout=datetime.timedelta(seconds=int(os.environ.get("OSB_DIST_TIMEOUT_S", "300"))))
     return dist
 
@@ -532,7 +535,7 @@ def run_reference(args):
         return
     w = make_workload(args.workload)
     if not os.path.exists(ORACLE_LIB):
-        emit_line({"impl": "reference", "unavailable": "oracle/_ref/liboracle_ref.so missing (built from /root/reference by __graft_entry__.build())"})
+        emit_line({"impl": "reference", "unavailable": "oracle/_ref/liboracle_ref.so missing (built from the reference sources by __graft_entry__.build())"})
         return
     d, meta = ensure_model(w)
     inputs = w.inputs(0)
@@ -548,8 +551,31 @@ def run_reference(args):
 
 
 # =====================================================================================================================
-# the B200 arm
+# the engine arm
 # =====================================================================================================================
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(dump_dir, workload, m):
+    """Every output tensor `m` hands its caller after the last run, as DIR/<workload>.<name>.npy in float32.  Above DUMP_LIMIT_BYTES in
+    all, each array keeps the same fixed seeded fraction of its flattened values."""
+    arrs = {}
+    for n in m.get_all_tensor_names():
+        t = m.get_tensor(n)
+        if t is None:
+            t = m.get_tensor_i64(n)
+        if t is not None:
+            arrs[n] = np.ascontiguousarray(np.asarray(t, dtype=np.float32))
+    total = sum(a.nbytes for a in arrs.values())
+    frac = DUMP_LIMIT_BYTES / total if total > DUMP_LIMIT_BYTES else 1.0
+    os.makedirs(dump_dir, exist_ok=True)
+    for n, a in arrs.items():
+        if frac < 1.0:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, max(1, int(a.size * frac)), replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(dump_dir, f"{workload}.{n}.npy"), a)
+
+
 def measure(w: Workload, args, dist, clocks=None):
     """value / e2e / roofline / parity for one single-model workload; returns the JSON line (rank 0) or None."""
     d, meta = ensure_model(w)
@@ -594,6 +620,9 @@ def measure(w: Workload, args, dist, clocks=None):
     gpu_ms = dist_max(dist, gpu_ms)
     ms_per_step = gpu_ms / args.steps
     value = WORLD * 1000.0 / ms_per_step
+    if getattr(args, "dump_outputs", None) and RANK == 0:
+        step_api(mv, later, None)      # one more replay of the timed graph on the same inputs, its outputs copied back
+        dump_outputs(args.dump_outputs, w.name, mv)
 
     # ---------------- supplementary: host inputs / outputs through the C ABI every step, weights resident ----------------
     e2e_resident = None
@@ -614,7 +643,7 @@ def measure(w: Workload, args, dist, clocks=None):
     else:
         e2e_resident = {"value": None, "note": f"failed: {e2e_r_err}"}
 
-    # ---------------- roofline leg: eager pass with per-launch CUDA events on the tcgen05 kernel ----------------
+    # ---------------- roofline leg: eager pass with per-launch CUDA events on the tensor-core kernel ----------------
     mv.lib.model_set_option(mv.h, b"b200_cuda_graph", 0)
     step_api(mv, inputs, w.out_name)
     mv.lib.osb_tc_profile(1)
@@ -630,12 +659,12 @@ def measure(w: Workload, args, dist, clocks=None):
     st_e = mv.stats()
     n_tc, tc_ms, tc_flops, tc_bytes = [float(x) for x in prof]
     achieved_tf = tc_flops / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else 0.0
-    roofline = {"bound": "tensor", "kernel": "tc_gemm_kernel + tc_pair_kernel (tcgen05 implicit-GEMM conv / GEMM: single-CTA and CTA-pair tiles, all launches of one step)",
+    roofline = {"bound": "tensor", "kernel": "tc_gemm_kernel (wgmma implicit-GEMM conv / GEMM, all launches of one step)",
                 "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf if peak_tf else None,
                 "peak_source": peak_src, "launches": int(n_tc), "kernel_ms_per_step": tc_ms, "flops_per_step": tc_flops,
                 "algorithmic_bytes_per_step": tc_bytes,
                 # share of the SAME eager, event-instrumented step (numerator and denominator carry the same per-launch event cost)
-                "share_of_step": tc_ms / float(st_e["last_gpu_ms"]) if st_e.get("last_gpu_ms") else None, "traffic": None}
+                "share_of_step": tc_ms / float(st_e["last_gpu_ms"]) if st_e.get("last_gpu_ms") else None}
     if w.hbm_bound or n_tc == 0:
         # weight-bandwidth-bound step (decode GEMVs): algorithmic bytes = every weight once + every graph input once, over the whole step
         in_bytes = sum(int(v.nbytes) // (2 if v.dtype == np.float32 else 1) for v in inputs.values())     # activations live as fp16
@@ -643,17 +672,7 @@ def measure(w: Workload, args, dist, clocks=None):
         ach = algo / (ms_per_step * 1e-3) / 1e9
         roofline = {"bound": "hbm", "kernel": "whole step (grouped gemv_panel / gemv_w8_panel + attention_decode + elementwise): weights and KV cache streamed once per token",
                     "achieved": ach, "peak": peak_bw, "unit": "GB/s", "frac": ach / peak_bw, "peak_source": peak_src.replace("sustained bf16 cuBLAS", "STREAM-style copy"),
-                    "algorithmic_bytes_per_step": algo, "traffic": None}
-    # DRAM traffic of the same kernel from the committed ncu pass (scripts/ncu_traffic.py): per launch, like `achieved`
-    for tname in ("r02_tc_traffic.json", "r01_tc_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", tname)
-        if w.name == "sd15_unet_fp16" and os.path.exists(tpath) and n_tc:
-            tj = json.load(open(tpath))
-            roofline["traffic"] = tj.get("dram_bytes_per_launch")
-            roofline["traffic_unit"] = "bytes/launch (ncu dram__bytes_read.sum + dram__bytes_write.sum, %d launches of one step; capture: profiles/%s%s)" % (
-                tj.get("launches", 0), tname, (", taken at commit " + tj["commit"]) if tj.get("commit") else "")
-            roofline["algorithmic_bytes_per_launch"] = tc_bytes / n_tc
-            break
+                    "algorithmic_bytes_per_step": algo}
     mv.close()
     del mv
 
@@ -710,7 +729,7 @@ def measure(w: Workload, args, dist, clocks=None):
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": w.dtype, "data": "synthetic",
         "config": {"workload": "%s: %d ops, %.0f M params, %.3f TFLOP/step; one sample per GPU" % (w.describe, meta["ops"], meta["params"] / 1e6, meta["flops"] / 1e12),
                    "weights": "value: " + value_mode + "; e2e: streamed pinned-host -> HBM ring every step",
-                   "l2": "per-step weight stream = %.2f GB >> 126 MB L2, no flush needed" % (meta["weight_bytes"] / 1e9), "parallelism": f"dp{WORLD} (rank r = sample r)"},
+                   "l2": "per-step weight stream = %.2f GB >> 50 MB L2, no flush needed" % (meta["weight_bytes"] / 1e9), "parallelism": f"dp{WORLD} (rank r = sample r)"},
         "clocks": clk,
         "e2e": {"value": e2e_value, "unit": w.unit, "ms_per_step": 1000.0 * e2e_s / args.steps, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "weight_ring_bytes": int(st["weight_ring_bytes"]), "largest_node_bytes": int(st["weight_largest_node_bytes"]),
@@ -719,7 +738,7 @@ def measure(w: Workload, args, dist, clocks=None):
         "e2e_resident_weights": e2e_resident,
         "parity": parity,
         "gpu_launches": launches_per_step * args.steps,
-        "gpu_launches_per_step": launches_per_step, "tcgen05_launches_per_step": int(st_e["tc_launches"]),
+        "gpu_launches_per_step": launches_per_step, "tensor_core_launches_per_step": int(st_e["tc_launches"]),
         "roofline": roofline,
     }
 
@@ -776,6 +795,7 @@ def main():
     ap.add_argument("--workload", default="sd15_unet_fp16", choices=WORKLOADS)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--all-configs", default=None, help="run every BASELINE workload and append one JSON line each to this file")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="after the timed steps, write the timed path's outputs to DIR/<workload>.<output>.npy (float32); by convention bench_dumps/<build>")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl != "reference" else args.warmup
 

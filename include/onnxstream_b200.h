@@ -10,7 +10,7 @@
  * model_set_option and model_add_tensor throw C++ exceptions across the boundary on error, as the reference does.
  *
  * Part 2 (model_ext_*, model_b200_*) covers Model members the reference's apps poke directly (src/onnxstream.h:944-968)
- * and B200-specific controls; none of them is needed by existing bindings.
+ * and engine-specific controls; none of them is needed by existing bindings.
  */
 #ifndef ONNXSTREAM_B200_H
 #define ONNXSTREAM_B200_H
@@ -60,7 +60,7 @@ char* model_b200_plan_summary(const char* model_text, int fp16_arithmetic, int f
 
 /* stats: [0] weight ring bytes, [1] peak live streamed weight bytes, [2] largest node footprint, [3] weight bytes streamed in the
  * last run, [4] HBM-resident cached weight bytes, [5] activation pool high-water, [6] input H2D bytes, [7] output D2H bytes,
- * [8] kernel launches, [9] tcgen05 launches, [10] steps executed, [11] ops fused away, [12] last run wall ms, [13] last run GPU ms,
+ * [8] kernel launches, [9] tensor-core launches, [10] steps executed, [11] ops fused away, [12] last run wall ms, [13] last run GPU ms,
  * [14] CUDA-graph replays.  Returns the number of fields available. */
 int   model_b200_get_stats(ModelContext* obj, double* out, int n);
 double model_b200_run_resident(ModelContext* obj, int steps);   /* replay the captured graph on device-resident inputs; CUDA-event ms, < 0 on error */

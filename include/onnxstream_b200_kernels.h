@@ -1,4 +1,4 @@
-/* onnxstream_b200_kernels.h -- internal C ABI between the C++ host (engine.cpp) and the hand-written sm_100a CUDA
+/* onnxstream_b200_kernels.h -- internal C ABI between the C++ host (engine.cpp) and the hand-written sm_90a CUDA
  * kernels.  Device pointers + explicit shapes/strides/dtype enums in, `int` status (cudaError_t value, 0 = OK) out,
  * no exceptions and no torch types across it.  Each entry point replaces one method of the reference's private
  * `class XnnPack` (src/onnxstream.cpp:657-2150) or one inline pthreadpool lambda of `Model::run()`
@@ -42,7 +42,7 @@ int osb_binary(int op, const void* a, const int64_t* a_strides, const void* b, c
  * out_offset + sum_k i_k * out_stride[k].  Covers XnnPack::transpose (src/onnxstream.cpp:1748-1809), Concat
  * (4140-4299), Split (5999-6119), Slice (6499-6695), Expand (7154-7351) and nearest Resize (6120-6315, in_div = scale). */
 /* fp32 Conv / MatMul / Gemm on the tensor cores (replaces XnnPack::convolution / matrix_multiply for float, src/onnxstream.cpp:1035-1534):
-   every fp32 operand is split into three bfloat16 parts (24 mantissa bits) and expanded 6x along K so that ONE tcgen05 contraction sums the
+   every fp32 operand is split into three bfloat16 parts (24 mantissa bits) and expanded 6x along K so that ONE tensor-core contraction sums the
    six significant cross products in its fp32 accumulator.  expand_cols: rows of length L -> rows of 6 L (GEMM A rows, [N][K] weights, NHWC
    pixels, OHWI taps); expand_rows: a [K][N] weight -> [6 K][N].  b_side: 0 for the A operand, 1 for the B operand (the segment orders pair up).
    The f32x launchers take the bf16 expansions and fp32 C / bias / residual; cudaErrorNotSupported (801) = shape outside the tensor-core path. */
@@ -103,13 +103,13 @@ int osb_gather_rows(const void* table, const int64_t* idx, void* out, int64_t n_
  * XnnPack::matrix_multiply / matrix_multiply_dynamic (src/onnxstream.cpp:929-1215) and the MatMul/Gemm branches
  * (4300-4375, 5669-5861).  stride_* are element strides between batches (0 = shared operand).
  * b_transposed: B[b] is stored N x K row-major.  Accumulation is fp32 for both dtypes.
- * `impl`: 0 = auto (tcgen05 when dtype == f16 and the shape is eligible), 1 = force the CUDA-core reference kernel,
- * 2 = force tcgen05 (returns an error if ineligible). */
+ * `impl`: 0 = auto (tensor cores when dtype == f16 and the shape is eligible), 1 = force the CUDA-core reference kernel,
+ * 2 = force the tensor-core kernel (returns an error if ineligible). */
 int osb_gemm(const void* A, const void* B, void* C, const void* bias, const void* residual,
              int64_t batch, int64_t M, int64_t N, int64_t K,
              int64_t stride_a, int64_t stride_b, int64_t stride_c, int b_transposed, int dtype, int impl, void* stream);
 
-/* `groups` (1..3) GEMMs C_g = A * B_g sharing A [M,K] and the shape, dense operands, no bias: one tcgen05 launch when the
+/* `groups` (1..3) GEMMs C_g = A * B_g sharing A [M,K] and the shape, dense operands, no bias: one tensor-core launch when the
  * problem qualifies (the q/k/v MatMuls of an attention block, src/onnxstream.cpp:4343-4664 run three times), else `groups`
  * ordinary launches. */
 int osb_gemm_grouped(const void* A, const void* const* B, void* const* C, int groups, int64_t M, int64_t N, int64_t K,
@@ -152,7 +152,7 @@ int osb_gemv_w8(const void* A, const void* Wq, void* C, const void* bias, const 
    shapes are outside the grouped kernels: launch them one by one. */
 int osb_gemv_grouped(const void* A, const void* const* B, void* const* C, const int64_t* N, const float* wscale, const int* wzp, int groups,
                      int64_t M, int64_t K, int wdtype, int dtype, void* stream);
-/* W8A8 on the tensor cores (tcgen05.mma.kind::i8, uint8 x uint8 -> int32): XnnPack::matrix_multiply<uint8_t,int32_t> / convolution for uint8
+/* W8A8 on the tensor cores (wgmma .u8, uint8 x uint8 -> int32): XnnPack::matrix_multiply<uint8_t,int32_t> / convolution for uint8
  * (src/onnxstream.cpp:1035-1215, 1292-1534) with XNNPACK's fp32 requantisation y = clamp(lrintf(acc * sx*sw/sy)) + zy.  The kernel multiplies raw
  * bytes and corrects with rowsum_x / colsum_w (osb_rowsum_u8: row sums of a [rows][cols] byte matrix; osb_colsum_u8: column sums of a [K][N] one);
  * a convolution runs on the image padded with the input zero point (osb_pad_sum_u8 also emits its per-pixel channel sums).  *_ok: TMA-addressable. */
@@ -191,8 +191,8 @@ int osb_attention(const void* q, const void* k, const void* v, const void* mask,
                   int64_t heads, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, float scale, int k_transposed,
                   int64_t kv_group, int dtype, void* stream);
 
-/* Fused flash-style multi-head attention on tcgen05 (fp16, d <= 64): q [T, heads*d] / k, v [Tk, heads*d] are read in place
- * from the projection buffers (row strides ld*), out [T, heads*d] is written in the merged layout; the score tile lives in TMEM.
+/* Fused flash-style multi-head attention on wgmma (fp16, d <= 64): q [T, heads*d] / k, v [Tk, heads*d] are read in place
+ * from the projection buffers (row strides ld*), out [T, heads*d] is written in the merged layout; the score tile lives in registers.
  * Covers the MatMul/Mul/Softmax/MatMul pattern plus the head split / merge around it (src/onnxstream.cpp:3576-3633, 6696-6929). */
 int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype);
 int osb_flash_attention(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
@@ -217,15 +217,17 @@ int osb_maxpool_nhwc(const void* x, void* y, int dtype, int64_t H, int64_t W, in
 /* Fill `n` bytes-worth of elements with a constant (ConstantOfShape, src/onnxstream.cpp:7543-7588). */
 int osb_fill(void* dst, int dtype, size_t n, float value, void* stream);
 
-/* 1 when the tcgen05/TMA GEMM path can take this problem (used by tests and the bench to assert the fast path ran). */
+/* 1 when the wgmma/TMA GEMM path can take this problem (used by tests and the bench to assert the fast path ran). */
 int osb_gemm_tc_eligible(int64_t M, int64_t N, int64_t K, int dtype);
 
-/* Per-launch timing of the tcgen05 GEMM/conv kernel (CUDA events on the launching stream; eager mode only).
+/* Tile decomposition of the tensor-core GEMM / conv: 0 = one CTA per 128 x 128 tile only, 1 = the default rule (single tiles: CTA pairs
+ * measured slower on the H100), 2 = CTA pairs (2-CTA clusters sharing the B tile through TMA multicast) wherever the shape is
+ * eligible.  Tests and A/B runs. */
+void osb_tc_set_pair_mode(int mode);
+
+/* Per-launch timing of the wgmma GEMM/conv kernel (CUDA events on the launching stream; eager mode only).
  * osb_tc_profile(1) starts recording, osb_tc_profile_read fills {launches, total ms, total FLOPs, total algorithmic bytes}. */
 void osb_tc_profile(int enable);
-/* Tile decomposition of the tcgen05 GEMM / conv: 0 = one CTA per 128 x bn tile only, 1 = cost model (default), 2 = the CTA-pair
- * kernel (tcgen05.mma.cta_group::2, 256 x bn tiles, TMA-store epilogue) wherever the shape is eligible.  Tests and A/B runs. */
-void osb_tc_set_pair_mode(int mode);
 int osb_tc_profile_read(double* out4);
 int osb_tc_profile_dump(char* buf, int cap);   /* one line per launch: M N K taps batch split conv ms gflop */
 

@@ -1,6 +1,6 @@
-"""In-tree build of libonnxstream_b200.so (hand-written sm_100a CUDA + C++ host) with nvcc/g++ -- no cmake, no JIT cache.
+"""In-tree build of libonnxstream_b200.so (hand-written sm_90a CUDA + C++ host) with nvcc/g++ -- no cmake, no JIT cache.
 
-The built library lives next to the sources (git-ignored, but it travels to the GPU box with the repo snapshot).
+The built library lives next to the sources (git-ignored).
 `python -m onnxstream_b200.build` rebuilds what changed; `--force` rebuilds everything.
 """
 from __future__ import annotations
@@ -12,7 +12,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-# Build variants for A/B experiments on the GPU box: OSB_BUILD_VARIANT=name OSB_NVCC_EXTRA="-DFOO" builds
+# Build variants for A/B experiments: OSB_BUILD_VARIANT=name OSB_NVCC_EXTRA="-DFOO" builds
 # csrc/libonnxstream_b200_<name>.so from csrc/build_<name>/ (the product library is the unnamed variant).
 VARIANT = os.environ.get("OSB_BUILD_VARIANT", "")
 OBJ = os.path.join(CSRC, "build" + ("_" + VARIANT if VARIANT else ""))
@@ -20,13 +20,27 @@ LIB = os.path.join(CSRC, "libonnxstream_b200" + ("_" + VARIANT if VARIANT else "
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CXX = os.environ.get("OSB_CXX", "/usr/bin/g++")
 
-CU_SOURCES = ["kernels_basic.cu", "kernels_gemm.cu", "gemm_tcgen05.cu", "attention_tcgen05.cu"]
+CU_SOURCES = ["kernels_basic.cu", "kernels_gemm.cu", "gemm_wgmma.cu", "attention_wgmma.cu"]
 CPP_SOURCES = ["engine.cpp", "engine_run.cpp", "capi.cpp", "comm.cpp", "workspace.cpp"]
 HEADERS = ["common.cuh", "engine.h", "engine_impl.h", "workspace.h", "../../include/onnxstream_b200_kernels.h", "../../include/onnxstream_b200.h"]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
               "-Xcompiler", "-fPIC", "-ccbin", CXX] + os.environ.get("OSB_NVCC_EXTRA", "").split()
 CXX_FLAGS = ["-std=c++17", "-O2", "-fPIC", "-I/usr/local/cuda/include", "-Wall", "-Wno-sign-compare", "-Wno-unused-function"]
+
+
+# where a read-only checkout of the reference (github.com/vitoplantamura/OnnxStream) is looked for: next to this repository, or at
+# /root/reference; ONNXSTREAM_REF_SRC (its src/ directory) overrides both
+REFERENCE_SRC_CANDIDATES = (os.path.join(os.path.dirname(os.path.dirname(HERE)), "reference", "src"), "/root/reference/src")
+
+
+def reference_src():
+    """The reference's src/ directory, or None: only the oracle, its YOLOv8n fixture and the C++ link test need it."""
+    env = os.environ.get("ONNXSTREAM_REF_SRC", "")
+    for ref in ((env,) if env else REFERENCE_SRC_CANDIDATES):
+        if os.path.isfile(os.path.join(ref, "onnxstream.cpp")):
+            return ref
+    return None
 
 
 def _newer(src_paths, target):
@@ -65,11 +79,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
         _run([NVCC, "-shared", "-o", LIB] + objs + ["-cudart", "static", "-ccbin", CXX, "-Xlinker", "--no-undefined", "-ldl", "-lpthread"])
     # keep the C++ drop-in link test (reference apps + compat_onnxstream.cpp) in step with the engine ABI
     link_script = os.path.join(os.path.dirname(HERE), "scripts", "link_reference_apps.sh")
-    compat_obj = os.path.join(os.path.dirname(HERE), "build", "link_test", "compat.o")
-    if not VARIANT and os.path.isdir("/root/reference/src") and os.path.exists(link_script) and _newer(hdrs + [os.path.join(CSRC, "compat_onnxstream.cpp"), LIB], compat_obj):
-        r = subprocess.run(["bash", link_script], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    compat_obj = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "link_test", "compat.o")
+    if not VARIANT and reference_src() and os.path.exists(link_script) and _newer(hdrs + [os.path.join(CSRC, "compat_onnxstream.cpp"), LIB], compat_obj):
+        r = subprocess.run(["bash", link_script], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=dict(os.environ, REF=reference_src()))
         if r.returncode != 0:
-            raise RuntimeError("link test (reference apps against the B200 engine) failed:\n" + r.stdout[-3000:])
+            raise RuntimeError("link test (reference apps against the engine) failed:\n" + r.stdout[-3000:])
     return LIB
 
 

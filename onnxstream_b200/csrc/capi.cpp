@@ -1,5 +1,5 @@
 // capi.cpp -- the drop-in C ABI: the 16 `model_*` entry points of the reference's FFI (src/exports.cpp:42-311) on top
-// of the B200 engine, plus `model_ext_*` / `model_b200_*` extensions for knobs the reference's apps set directly on
+// of the engine, plus `model_ext_*` / `model_b200_*` extensions for knobs the reference's apps set directly on
 // public Model members (src/onnxstream.h:944-968).  Conventions are the reference's: opaque context pointer, borrowed
 // NUL-terminated strings in, malloc'd strings/structs out (freed with model_free_buffer), raw pointers into
 // engine-owned storage for tensor uploads, errors as malloc'd messages (model_read_file / model_run_2) or C++
@@ -297,12 +297,12 @@ int model_b200_set_comm(ModelContext* obj, void* nccl_comm, int rank, int nranks
     return 0;
 }
 
-// cudaProfilerStart/Stop for `ncu --profile-from-start off` (profiles/ recipes)
+// cudaProfilerStart/Stop around a region of interest (profilers started with capture off)
 void model_b200_profiler(int start)
 {
     if (start) cudaProfilerStart(); else cudaProfilerStop();
 }
 
-const char* model_b200_version() { return "onnxstream_b200 0.1 (sm_100a)"; }
+const char* model_b200_version() { return "onnxstream_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the sm_100a kernels.
+// common.cuh -- shared device helpers for the sm_90a kernels.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -26,8 +26,8 @@ static inline int launched(int tensor_core = 0)
 // latency and prologue of kernel i+1 behind the tail of kernel i (CUDA graphs keep the programmatic edges).
 __device__ __forceinline__ void osb_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void osb_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-// OSB_PDL_LATE (build variant): short kernels do not trigger at all (the implicit trigger at exit stands), the tcgen05 kernels
-// trigger once their last tile's main loop has been issued -- so dependents never take SM slots from CTAs that still have work.
+// OSB_PDL_LATE (build variant): short kernels do not trigger at all (the implicit trigger at exit stands), the tensor-core kernels
+// trigger once their producer has issued the last tile's loads -- so dependents never take SM slots from CTAs that still have work.
 #ifdef OSB_PDL_LATE
 __device__ __forceinline__ void osb_pdl_trigger_entry() {}
 __device__ __forceinline__ void osb_pdl_trigger_late() { osb_pdl_trigger(); }
@@ -39,17 +39,33 @@ __device__ __forceinline__ void osb_pdl_prologue() { osb_pdl_trigger_entry(); os
 
 extern "C" int osb_pdl_enabled(void);
 
+// cluster > 1: thread-block clusters of `cluster` consecutive CTAs along x (grid.x must be a multiple of it)
 template <typename... KArgs, typename... Args>
-static inline void osb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args)
+static inline void osb_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, unsigned cluster, Args&&... args)
 {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchAttribute attr[2];
+    int n = 0;
+    if (osb_pdl_enabled()) {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n].val.programmaticStreamSerializationAllowed = 1;
+        n++;
+    }
+    if (cluster > 1) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n].val.clusterDim.x = cluster; attr[n].val.clusterDim.y = 1; attr[n].val.clusterDim.z = 1;
+        n++;
+    }
     cfg.attrs = attr;
-    cfg.numAttrs = osb_pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = n;
     cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);   // errors surface through launched() / cudaGetLastError
+}
+
+template <typename... KArgs, typename... Args>
+static inline void osb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args)
+{
+    osb_launch_cluster(kernel, grid, block, smem, st, 1u, std::forward<Args>(args)...);
 }
 
 // Cooperative launch: the driver gang-schedules the grid (every CTA resident at once, or the launch fails with
@@ -68,10 +84,13 @@ static inline void osb_launch_coop(void (*kernel)(KArgs...), dim3 grid, dim3 blo
     cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
+// streaming multiprocessors of an H100 SXM: caps the grids of the grid-stride kernels (the tensor-core launchers query the device)
+constexpr int OSB_SMS = 132;
+
 static inline int grid_for(size_t work_items, int threads)
 {
     size_t blocks = (work_items + threads - 1) / threads;
-    size_t cap = 148ull * 16;  // persistent-ish: at most 16 CTAs per SM, grid-stride loops cover the rest
+    size_t cap = (size_t)OSB_SMS * 16;  // persistent-ish: at most 16 CTAs per SM, grid-stride loops cover the rest
     if (blocks < 1) blocks = 1;
     return (int)(blocks < cap ? blocks : cap);
 }

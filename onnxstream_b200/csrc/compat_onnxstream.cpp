@@ -15,7 +15,7 @@
 // (on_init once per weight in order on the first init(), on_restart before later runs, src/onnxstream.cpp:3499-3548);
 // tensors pushed twice under one name become m_batch siblings (src/onnxstream.cpp:3040-3050); after run() m_data holds the
 // graph outputs and m_extra_outputs as float32 NCHW (src/onnxstream.cpp:8217-8263).
-#include "onnxstream.h"   // the reference's header, found through -I/root/reference/src
+#include "onnxstream.h"   // the reference's header, found through -I<reference checkout>/src
 
 #include "engine_impl.h"
 

@@ -1,4 +1,4 @@
-// engine.cpp -- infrastructure of the B200 engine: device pool, model.txt parser, weight sources, the streaming
+// engine.cpp -- infrastructure of the engine: device pool, model.txt parser, weight sources, the streaming
 // HBM weight ring.  The op interpreter lives in engine_run.cpp.
 #include "engine_impl.h"
 
@@ -54,8 +54,8 @@ const char* dtype_name(DType t)
 // ================================================================================================================
 // NUMA-local pinned memory
 // ================================================================================================================
-// On a two-socket host a pinned buffer that lands on the socket the GPU is NOT attached to streams at ~30 GB/s instead of
-// ~47 GB/s (measured on the B200 boxes: the whole streaming step is PCIe-bound, so that is a 1.5x difference end to end).
+// On a two-socket host a pinned buffer that lands on the socket the GPU is NOT attached to streams markedly slower over PCIe
+// (and the whole streaming step is PCIe-bound).
 // Pages are allocated on the node of the thread that calls cudaHostAlloc, so the call runs with the thread temporarily bound
 // to the CPUs local to the current device (/sys/bus/pci/devices/<bdf>/local_cpulist); the previous affinity is restored on
 // scope exit.  OSB_NUMA_BIND=0 disables it; any failure degrades to a plain allocation.

@@ -1,4 +1,4 @@
-// engine.h -- B200-native per-node execution engine behind OnnxStream's Model / WeightsProvider surface.
+// engine.h -- H100-native per-node execution engine behind OnnxStream's Model / WeightsProvider surface.
 //
 // The reference executes a text graph op by op on the CPU (Model::run, src/onnxstream.cpp:3550-8269), fetching each
 // node's weights from a WeightsProvider (src/onnxstream.h:266-900) right before use.  This engine keeps exactly that
@@ -193,13 +193,13 @@ public:
     bool range_data_calibrate = false;     // m_range_data_calibrate (src/onnxstream.h:964): record every op output's percentile range
     int cpu_threads = 0;                   // the reference's pool size (Model(threads_count)): it partitions the percentile chunks
 
-    // --- B200-specific knobs (set through model_set_option("b200_*")) ---
+    // --- engine-specific knobs (set through model_set_option("b200_*")) ---
     bool resident_weights = false;   // keep converted weights in HBM after the first run (upper bound; "--ram" analogue)
     bool use_cuda_graph = false;     // capture run() once and replay
     bool fuse_nodes = true;          // GroupNorm/LayerNorm/GELU/SiLU/bias/residual fusions
     bool keep_nhwc = true;           // keep conv trunks channel-last instead of transposing around every Conv
-    int gemm_impl = 0;               // 0 auto, 1 force CUDA-core kernels, 2 force tcgen05
-    bool flash_attention = true;     // fused tcgen05 attention for d <= 64 (else two GEMMs around a softmax)
+    int gemm_impl = 0;               // 0 auto, 1 force CUDA-core kernels, 2 force the tensor-core kernel
+    bool flash_attention = true;     // fused wgmma attention for d <= 64 (else two GEMMs around a softmax)
     double ring_factor = 1.0;        // weight ring capacity = ring_factor * largest node footprint
     bool keep_inputs = false;        // graph inputs stay in HBM after a run; a later run that does not push a name again reuses the device copy
                                      // (a device-resident KV cache for fixed-shape decode steps: only the new token's ids cross PCIe)

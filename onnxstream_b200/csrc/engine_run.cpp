@@ -930,8 +930,8 @@ struct Engine::Impl {
             largest_node = std::max(largest_node, node_bytes);
         }
         is_side.clear(); side_deps.clear(); kv_side.clear();
-        // opt-in (OSB_SIDE_BRANCH=1): measured on B200 inside the captured UNet graph, 112 steps on the side branch changed the replay time
-        // by +0.02 ms (5.505 vs 5.486 ms, profiles/r02_ab_step_e2e.txt) -- the branch does not shorten the critical path in practice
+        // opt-in (OSB_SIDE_BRANCH=1): inside the captured UNet graph the 112 latent-independent steps on a side branch did not shorten
+        // the critical path in practice
         static const bool side_on = [] { const char* e = getenv("OSB_SIDE_BRANCH"); return e && e[0] == '1'; }();
         if (side_on && E.fuse_nodes) plan_side_branch_impl();
     }
@@ -1227,7 +1227,7 @@ void Engine::Impl::op_conv(size_t oi, const Tensor* residual, size_t out_op)
         else if (a.first == "strides") strides = parse_ints(a.second);
         else fail(op, "unrecognized attribute: " + a.first + ".");
     }
-    if (E.use_nchw_convs) fail(op, "m_use_nchw_convs is not supported by the B200 engine (file-backed conv weights are NHWC, src/onnxstream.cpp:2686-2689).");
+    if (E.use_nchw_convs) fail(op, "m_use_nchw_convs is not supported by the engine (file-backed conv weights are NHWC, src/onnxstream.cpp:2686-2689).");
     bool is1d = dil.size() == 1;
     if (is1d) {
         dil.push_back(1); ks.push_back(1);
@@ -1287,7 +1287,7 @@ void Engine::Impl::op_conv(size_t oi, const Tensor* residual, size_t out_op)
         y = make(DType::u8, { 1, Cout, Ho, Wo }, Layout::nhwc);
         y.scale = oscale; y.zero_point = ozp;
         if (E.gemm_impl != 1 && osb_qu8_tc_conv_ok(Cin, Cout, Ho, Wo, kh, kw, stride, x.data(), w.data(), y.mdata())) {
-            // tensor cores (tcgen05.mma.kind::i8): the image is padded once with the input zero point -- XNNPACK's padding value, which
+            // tensor cores (wgmma .u8): the image is padded once with the input zero point -- XNNPACK's padding value, which
             // TMA's zero fill cannot produce -- and the conv runs un-padded on it; zero-point terms are applied in the epilogue
             const int64_t Hp = (Ho - 1) * stride + kh, Wp = (Wo - 1) * stride + kw;
             DevPtr xp = pool().alloc((size_t)(Hp * Wp * Cin)), psum = pool().alloc((size_t)(Hp * Wp) * 4), csum = pool().alloc((size_t)Cout * 4);
@@ -1391,7 +1391,7 @@ void Engine::Impl::op_matmul(size_t oi, const Tensor* bias, const Tensor* residu
         for (int64_t i = 0; i < n; i++) {
             const uint8_t* ai = (const uint8_t*)a.data() + i * M * Kd; const uint8_t* bi = (const uint8_t*)b.data() + i * stride_b; uint8_t* yi = (uint8_t*)y.mdata() + i * M * N;
             if (E.gemm_impl != 1 && osb_qu8_tc_gemm_ok(M, N, Kd, ai, bi, yi)) {
-                // tensor cores (tcgen05.mma.kind::i8) on the raw bytes; row sums of x and column sums of w feed the zero-point terms
+                // tensor cores (wgmma .u8) on the raw bytes; row sums of x and column sums of w feed the zero-point terms
                 DevPtr rsum = pool().alloc((size_t)M * 4), csum = pool().alloc((size_t)N * 4);
                 ck(osb_rowsum_u8(ai, rsum->ptr, M, Kd, st), "osb_rowsum_u8");
                 ck(osb_colsum_u8(bi, csum->ptr, Kd, N, st), "osb_colsum_u8");
@@ -1841,7 +1841,7 @@ void Engine::Impl::op_resize(size_t oi)
     }
     if (ctm != "asymmetric" || mode != "nearest" || nm != "floor") fail(op, "one or more attributes are not supported (not implemented).");
     int64_t sy = (int64_t)scales[2], sx = (int64_t)scales[3];
-    if ((float)sy != scales[2] || (float)sx != scales[3] || sy < 1 || sx < 1) fail(op, "non-integer resize scales are not implemented in the B200 engine.");
+    if ((float)sy != scales[2] || (float)sx != scales[3] || sy < 1 || sx < 1) fail(op, "non-integer resize scales are not implemented in the engine.");
     int64_t C = x.shape[1], H = x.shape[2], W = x.shape[3];
     Tensor y;
     if (x.layout == Layout::nhwc && E.keep_nhwc) {
@@ -2074,7 +2074,7 @@ void Engine::Impl::op_misc_host(size_t oi)
         push(oi, 0, mk_i64(std::move(v), { n }));
     } else if (op.type == "Less" || op.type == "Greater" || op.type == "Equal" || op.type == "And") {
         Tensor a = in(oi, 0), b = in(oi, 1);
-        if (a.type != DType::i64 || b.type != DType::i64) fail(op, "only int64 operands are implemented in the B200 engine.");
+        if (a.type != DType::i64 || b.type != DType::i64) fail(op, "only int64 operands are implemented in the engine.");
         size_t na = a.i64->size(), nb = b.i64->size(), n = std::max(na, nb);
         if (!(na == nb || na == 1 || nb == 1)) {
             // outer-product style broadcast [n,1] vs [1,m] / [m]
@@ -2415,7 +2415,7 @@ void Engine::Impl::fused_mha(const Step& s)
     }
 
     if (use_flash) {
-        // one kernel: QK^T -> online softmax -> PV with the score tile in TMEM
+        // one kernel: QK^T -> online softmax -> PV with the score tile in registers
         ck(osb_flash_attention(ql.data(), C, kl.data(), C, vl.data(), C, out.mdata(), C, h, T, Tk, d, scale, st), "osb_flash_attention");
         push(i + 19, 0, out);
         return;

@@ -1,4 +1,4 @@
-// gemm_i8.cuh -- W8A8 on the tensor cores: `tcgen05.mma.kind::i8`, uint8 x uint8 -> int32 in TMEM (included by gemm_tcgen05.cu).
+// gemm_i8.cuh -- W8A8 on the tensor cores: `wgmma ... .s32.u8.u8`, uint8 x uint8 -> int32 in registers (included by gemm_wgmma.cu).
 //
 // Replaces XnnPack::matrix_multiply<uint8_t,int32_t> / convolution for T = uint8_t (src/onnxstream.cpp:1035-1215, 1292-1534; the reference
 // drives XNNPACK's qu8 GEMM / conv with the parameters of Qu8MatMulData / Qu8ConvData, 1025-1033) for the shapes TMA can address
@@ -13,20 +13,23 @@
 // out-of-bounds elements with 0: the host therefore pads the NHWC image once (value zx, kernel in this file) and the conv runs
 // un-padded on it, so every tap of every output pixel is a real byte and rowsum_x[m] is the sum of kh*kw per-pixel channel sums.
 //
-// Structure = tc_gemm_kernel (warp 0 TMA producer, warp 1 MMA issuer, warps 2..5 epilogue, 2 accumulator stages in TMEM), with
-// 128-byte k-blocks = 128 elements, UMMA_K = 32.  A is K-major; B is K-major (OHWI conv weights) or MN-major ([K,N] MatMul weights --
-// MN-major is valid for 8-bit integer operands, cute/arch/mma_sm100_desc.hpp InstrDescriptor::b_major_).
+// Structure = tc_gemm_kernel (warp 0 TMA producer, warpgroups 1 and 2 MMA + epilogue on 64 rows each), with 128-byte k-blocks = 128
+// elements, m64n128k32 MMAs.  A is K-major; B is K-major (OHWI conv weights) or MN-major ([K,N] MatMul weights).  wgmma reads 8-bit
+// operands K-major only, so an MN-major B k-block lands in a staging buffer and warps 1..3 of the producer warpgroup transpose it
+// into the K-major swizzled stage the MMAs read.
 
 namespace i8k {
 
 constexpr int I8_BLOCK_K = 128;        // elements = bytes: one 128B swizzle row
-constexpr int I8_UMMA_K = 32;
+constexpr int I8_WG_K = 32;
 constexpr int I8_STAGES = 4;
-constexpr int I8_SMEM = I8_STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 + 256;
+constexpr int I8_STAGE_BYTES = A_STAGE_BYTES + 2 * B_STAGE_BYTES;   // A, B, the MN-major staging buffer
+constexpr int I8_SMEM = I8_STAGES * I8_STAGE_BYTES + 1024 + 256;
+constexpr int TRANSPOSE_THREADS = 96;
 
 struct I8Params {
     int M, N, K;                 // GEMM view (conv: M = Ho*Wo, K = Cin per tap)
-    int m_tiles, n_tiles, bn;
+    int m_tiles, n_tiles;
     int b_kmajor;
     int taps, kw, Wo, Ho, bw, bh, tiles_x, k_blocks_per_tap, stride;
     int Wp;                      // conv: width of the zero-point-padded image (rows of `psum`)
@@ -40,16 +43,6 @@ struct I8Params {
     long long ldc;
 };
 
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc_i8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const I8Params p)
 {
@@ -58,12 +51,11 @@ tc_i8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ 
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + I8_STAGES * A_STAGE_BYTES;
-    uint64_t* bars = (uint64_t*)(smem + I8_STAGES * (A_STAGE_BYTES + B_STAGE_BYTES));
-    uint64_t* full = bars;
-    uint64_t* empty = bars + I8_STAGES;
-    uint64_t* acc_full = bars + 2 * I8_STAGES;
-    uint64_t* acc_empty = acc_full + ACC_STAGES;
-    uint32_t* tmem_slot = (uint32_t*)(acc_empty + ACC_STAGES);
+    uint8_t* smem_stg = smem_b + I8_STAGES * B_STAGE_BYTES;
+    uint64_t* bars = (uint64_t*)(smem + I8_STAGES * I8_STAGE_BYTES);
+    uint64_t* full = bars;                    // [I8_STAGES] A and (K-major) B landed / (MN-major) B transposed
+    uint64_t* empty = bars + I8_STAGES;       // [I8_STAGES] consumers are done with the stage
+    uint64_t* stg_full = empty + I8_STAGES;   // [I8_STAGES] MN-major B landed in the staging buffer
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 0 && lane == 0) {
@@ -71,18 +63,14 @@ tc_i8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ 
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
     }
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < I8_STAGES; i++) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < ACC_STAGES; i++) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 4 * 32); }
+        for (int i = 0; i < I8_STAGES; i++) {
+            mbar_init(&full[i], p.b_kmajor ? 1 : 2);   // MN-major: the TMA of A and the transposers' arrival
+            mbar_init(&empty[i], CONSUMER_THREADS);
+            mbar_init(&stg_full[i], 1);
+        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     osb_pdl_wait();
 
     const int total_tiles = p.m_tiles * p.n_tiles;
@@ -90,12 +78,11 @@ tc_i8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ 
 
     if (warp == 0) {
         // ===================== TMA producer =====================
-        const uint32_t sa0 = smem_u32(smem_a), sb0 = smem_u32(smem_b);
-        const uint32_t tx_bytes = A_STAGE_BYTES + (p.b_kmajor ? (uint32_t)p.bn * I8_BLOCK_K : (uint32_t)B_STAGE_BYTES);
+        const uint32_t sa0 = smem_u32(smem_a), sb0 = smem_u32(smem_b), sg0 = smem_u32(smem_stg);
         int stage = 0; uint32_t phase = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int mt = tile % p.m_tiles, nt = tile / p.m_tiles;
-            const int n0 = nt * p.bn, m0 = mt * BLOCK_M;
+            const int n0 = nt * BLOCK_N, m0 = mt * BLOCK_M;
             int y0 = 0, x0 = 0;
             if (p.bh > 0) { y0 = (mt / p.tiles_x) * p.bh; x0 = (mt % p.tiles_x) * p.bw; }
             int tap = 0, kcb = 0, ky = 0, kx = 0;
@@ -103,121 +90,129 @@ tc_i8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ 
             for (int kb = 0; kb < k_blocks; kb++) {
                 mbar_wait(&empty[stage], phase ^ 1);
                 if (elect_one()) {
-                    mbar_expect_tx(&full[stage], tx_bytes);
                     const int kc = kcb * I8_BLOCK_K;
-                    const uint32_t sa = sa0 + stage * A_STAGE_BYTES, sb = sb0 + stage * B_STAGE_BYTES;
+                    const uint32_t sa = sa0 + stage * A_STAGE_BYTES;
+                    const int kglob = tap * p.K + kc;
+                    if (p.b_kmajor) {
+                        mbar_expect_tx(&full[stage], A_STAGE_BYTES + B_STAGE_BYTES);
+                        tma_load_3d_s(sb0 + stage * B_STAGE_BYTES, &map_b, &full[stage], kglob, n0, 0);
+                    } else {
+                        mbar_expect_tx(&full[stage], A_STAGE_BYTES);
+                        mbar_expect_tx(&stg_full[stage], B_STAGE_BYTES);
+                        tma_load_3d_s(sg0 + stage * B_STAGE_BYTES, &map_b, &stg_full[stage], n0, kglob, 0);   // 128 columns x 128 k-rows
+                    }
                     if (p.bh > 0) tma_load_3d_s(sa, &map_a, &full[stage], kc, ax + kx, ay + ky);
                     else tma_load_3d_s(sa, &map_a, &full[stage], kc, m0, 0);
-                    const int kglob = tap * p.K + kc;
-                    if (p.b_kmajor) tma_load_3d_s(sb, &map_b, &full[stage], kglob, n0, 0);
-                    else tma_load_3d_s(sb, &map_b, &full[stage], n0, kglob, 0);      // one box: 128 columns (128 B) x 128 k-rows
                 }
                 __syncwarp();
                 if (++kcb == p.k_blocks_per_tap) { kcb = 0; tap++; if (++kx == p.kw) { kx = 0; ky++; } }
                 if (++stage == I8_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        uint32_t idesc = 0;
-        idesc |= 2u << 4;                                    // D = S32
-        idesc |= 0u << 7;                                    // A = unsigned 8 bit
-        idesc |= 0u << 10;                                   // B = unsigned 8 bit
-        idesc |= (uint32_t)(p.b_kmajor ? 0 : 1) << 16;       // B major
-        idesc |= (uint32_t)(p.bn >> 3) << 17;
-        idesc |= (uint32_t)(BLOCK_M >> 4) << 24;
-        const uint64_t adesc0 = make_smem_desc(smem_u32(smem_a), 16, 1024);
-        const uint64_t bdesc0 = make_smem_desc(smem_u32(smem_b), 16, 1024);     // MN-major: a single 128-column atom, 8-row k-groups 1024 B apart
-        const uint32_t a_kstep = I8_UMMA_K >> 4;                                  // 32 bytes along K
-        const uint32_t b_kstep = p.b_kmajor ? (I8_UMMA_K >> 4) : ((I8_UMMA_K * 128) >> 4);
-        int stage = 0; uint32_t phase = 0;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            mbar_wait(&acc_empty[acc], acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BLOCK_N);
-            for (int kb = 0; kb < k_blocks; kb++) {
-                mbar_wait(&full[stage], phase);
-                tc_fence_after();
-                const uint64_t adesc = adesc0 + (uint64_t)(stage * (A_STAGE_BYTES >> 4));
-                const uint64_t bdesc = bdesc0 + (uint64_t)(stage * (B_STAGE_BYTES >> 4));
-                if (elect_one()) {
-#pragma unroll
-                    for (int k = 0; k < I8_BLOCK_K / I8_UMMA_K; k++)
-                        umma_i8(tmem_d, adesc + (uint64_t)(k * a_kstep), bdesc + (uint64_t)(k * b_kstep), idesc, (kb | k) != 0 ? 1u : 0u);
-                    umma_commit(&empty[stage]);
-                    if (kb == k_blocks - 1) umma_commit(&acc_full[acc]);
-                }
-                __syncwarp();
-                if (++stage == I8_STAGES) { stage = 0; phase ^= 1; }
-            }
-            if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-        }
         osb_pdl_trigger_late();
-    } else {
-        // ===================== epilogue: zero-point corrections + fp32 requantisation =====================
-        const int q = warp & 3;
-        int acc = 0; uint32_t acc_phase = 0;
+    } else if (warp < 4) {
+        // ===================== transposers (MN-major B only): staging [k][n] -> B stage [n][k], both 128B-swizzled =====================
+        if (p.b_kmajor) return;
+        const int t = (int)threadIdx.x - 32;
+        int stage = 0; uint32_t phase = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const int mt = tile % p.m_tiles, nt = tile / p.m_tiles;
-            const int n0 = nt * p.bn;
-            const int n_end = min(p.N, n0 + p.bn);
-            const int row_in_tile = q * 32 + lane;
-            long long out_row; bool row_ok; int rs = 0;
-            if (p.bh > 0) {
-                const int y = (mt / p.tiles_x) * p.bh + row_in_tile / p.bw, x = (mt % p.tiles_x) * p.bw + row_in_tile % p.bw;
-                row_ok = y < p.Ho && x < p.Wo;
-                out_row = (long long)y * p.Wo + x;
-                if (row_ok) {
-                    const int kh = p.taps / p.kw;
-                    for (int ky = 0; ky < kh; ky++)
-                        for (int kx = 0; kx < p.kw; kx++) rs += p.rsum[(long long)(y * p.stride + ky) * p.Wp + (x * p.stride + kx)];
-                }
-            } else {
-                const int m = mt * BLOCK_M + row_in_tile;
-                row_ok = m < p.M;
-                out_row = m;
-                if (row_ok) rs = p.rsum[m];
-            }
-            const int row_term = p.kzz - p.zw * rs;
-            mbar_wait(&acc_full[acc], acc_phase);
-            tc_fence_after();
-            uint8_t* crow = p.C + out_row * p.ldc;
-#pragma unroll 1
-            for (int c = 0; c < p.bn; c += 32) {
-                if (n0 + c >= n_end) break;
-                uint32_t v[32];
-                tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BLOCK_N + c), v);
-                if (row_ok) {
+            for (int kb = 0; kb < k_blocks; kb++) {
+                mbar_wait(&stg_full[stage], phase);
+                const uint8_t* stg = smem_stg + stage * B_STAGE_BYTES;
+                uint8_t* dst = smem_b + stage * B_STAGE_BYTES;
+                for (int n = t; n < BLOCK_N; n += TRANSPOSE_THREADS) {
 #pragma unroll
-                    for (int j = 0; j < 32; j += 16) {
-                        const int n = n0 + c + j;
-                        if (n >= n_end) break;            // N % 16 == 0
-                        uint32_t packed[4];
+                    for (int c = 0; c < I8_BLOCK_K / 16; c++) {
+                        uint32_t w[4];
 #pragma unroll
-                        for (int t = 0; t < 16; t++) {
-                            int a = (int)v[j + t] + row_term - p.zx * __ldg(p.csum + n + t);
-                            if (p.bias) a += __ldg(p.bias + n + t);
-                            float f = (float)a * p.requant;
-                            f = fminf(fmaxf(f, (float)(0 - p.zy)), (float)(255 - p.zy));
-                            const uint32_t o = (uint32_t)((int)rintf(f) + p.zy) & 0xFFu;
-                            if ((t & 3) == 0) packed[t >> 2] = o; else packed[t >> 2] |= o << (8 * (t & 3));
+                        for (int q = 0; q < 4; q++) {
+                            uint32_t v = 0;
+#pragma unroll
+                            for (int e = 0; e < 4; e++) {
+                                const int k = 16 * c + 4 * q + e;   // row k of the staging tile: 16-byte unit (n / 16) sits at unit (n / 16) ^ (k % 8)
+                                v |= (uint32_t)stg[k * 128 + ((((n >> 4) ^ (k & 7))) << 4) + (n & 15)] << (8 * e);
+                            }
+                            w[q] = v;
                         }
-                        *reinterpret_cast<uint4*>(crow + n) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
+                        *reinterpret_cast<uint4*>(dst + n * 128 + ((c ^ (n & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
                     }
                 }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor cores
+                asm volatile("bar.sync 2, %0;" ::"n"(TRANSPOSE_THREADS) : "memory");
+                if (t == 0) mbar_arrive(&full[stage]);
+                if (++stage == I8_STAGES) { stage = 0; phase ^= 1; }
             }
-            tc_fence_before();
-            mbar_arrive(&acc_empty[acc]);
-            if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+    } else {
+        // ===================== consumers: MMA + zero-point corrections + fp32 requantisation =====================
+        const int wg = (warp >> 2) - 1;
+        const uint64_t adesc0 = make_smem_desc(smem_u32(smem_a) + wg * (BLOCK_M / 2) * 128, 16, 1024);
+        const uint64_t bdesc0 = make_smem_desc(smem_u32(smem_b), 16, 1024);
+        const uint32_t kstep = I8_WG_K >> 4;                                      // 32 bytes along K, both operands
+        const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int cq = 2 * (lane & 3);
+        int stage = 0; uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const int mt = tile % p.m_tiles, nt = tile / p.m_tiles;
+            const int n0 = nt * BLOCK_N;
+            const int n_end = min(p.N, n0 + BLOCK_N);
+            int32_t acc[64];
+#pragma unroll
+            for (int i = 0; i < 64; i++) acc[i] = 0;
+            int prev = -1;
+            for (int kb = 0; kb < k_blocks; kb++) {
+                mbar_wait(&full[stage], phase);
+                const uint64_t adesc = adesc0 + (uint64_t)(stage * (A_STAGE_BYTES >> 4));
+                const uint64_t bdesc = bdesc0 + (uint64_t)(stage * (B_STAGE_BYTES >> 4));
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < I8_BLOCK_K / I8_WG_K; k++) wgmma_m64n128k32_u8(acc, adesc + (uint64_t)(k * kstep), bdesc + (uint64_t)(k * kstep), 1u);
+                wgmma_commit();
+                if (prev >= 0) { wgmma_wait<1>(); mbar_arrive(&empty[prev]); }
+                prev = stage;
+                if (++stage == I8_STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            mbar_arrive(&empty[prev]);
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int row_in_tile = r_lo + 8 * h;
+                long long out_row; bool row_ok; int rs = 0;
+                if (p.bh > 0) {
+                    const int y = (mt / p.tiles_x) * p.bh + row_in_tile / p.bw, x = (mt % p.tiles_x) * p.bw + row_in_tile % p.bw;
+                    row_ok = y < p.Ho && x < p.Wo;
+                    out_row = (long long)y * p.Wo + x;
+                    if (row_ok) {
+                        const int kh = p.taps / p.kw;
+                        for (int ky = 0; ky < kh; ky++)
+                            for (int kx = 0; kx < p.kw; kx++) rs += p.rsum[(long long)(y * p.stride + ky) * p.Wp + (x * p.stride + kx)];
+                    }
+                } else {
+                    const int m = mt * BLOCK_M + row_in_tile;
+                    row_ok = m < p.M;
+                    out_row = m;
+                    if (row_ok) rs = p.rsum[m];
+                }
+                if (!row_ok) continue;
+                const int row_term = p.kzz - p.zw * rs;
+                uint8_t* crow = p.C + out_row * p.ldc;
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; j++) {
+                    const int n = n0 + 8 * j + cq;
+                    if (n >= n_end) break;            // N % 16 == 0: both columns of the pair are inside
+                    uint32_t o2 = 0;
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        int a = acc[4 * j + 2 * h + e] + row_term - p.zx * __ldg(p.csum + n + e);
+                        if (p.bias) a += __ldg(p.bias + n + e);
+                        float f = (float)a * p.requant;
+                        f = fminf(fmaxf(f, (float)(0 - p.zy)), (float)(255 - p.zy));
+                        o2 |= ((uint32_t)((int)rintf(f) + p.zy) & 0xFFu) << (8 * e);
+                    }
+                    *reinterpret_cast<uint16_t*>(crow + n) = (uint16_t)o2;
+                }
+            }
+        }
     }
 }
 

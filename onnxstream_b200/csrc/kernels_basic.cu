@@ -1,4 +1,4 @@
-// kernels_basic.cu -- bandwidth-bound node kernels for sm_100a: dtype conversion, unary / broadcasting binary
+// kernels_basic.cu -- bandwidth-bound node kernels for sm_90a: dtype conversion, unary / broadcasting binary
 // elementwise, strided copies (transpose / concat / slice / expand / nearest resize), softmax, InstanceNorm,
 // fused GroupNorm(+SiLU), fused LayerNorm, ReduceMean, row gather.  Each replaces an XnnPack method or an inline
 // pthreadpool lambda of the reference's Model::run(); see include/onnxstream_b200_kernels.h for file:line citations.
@@ -867,7 +867,7 @@ __global__ void rms_norm_kernel(const TI* __restrict__ x, const TW* __restrict__
 }
 
 // few rows (a decode step has one): a whole CTA per row -- 256 threads, 4 independent loads each per pass, block reduction -- instead of one
-// warp walking the row with one load in flight (22 us for 2048 columns, ncu r02_launches_llama.csv)
+// warp walking the row with one load in flight
 template <typename TI, typename TW, typename TO>
 __global__ void __launch_bounds__(256) rms_norm_block_kernel(const TI* __restrict__ x, const TW* __restrict__ w, TO* __restrict__ y, int cols, float eps)
 {
@@ -1104,7 +1104,7 @@ int osb_binary(int op, const void* a, const int64_t* as, const void* b, const in
     return (int)cudaErrorInvalidValue;
 }
 
-// ---- fp32 -> bf16 triple split, expanded along K for the tensor-core fp32 path (gemm_tcgen05.cu: osb_tc_gemm_f32x) -----------------
+// ---- fp32 -> bf16 triple split, expanded along K for the tensor-core fp32 path (gemm_wgmma.cu: osb_tc_gemm_f32x) -----------------
 // x = h + m + l, h = bf16(x), m = bf16(x - h), l = bf16(x - h - m).  A side: segments [h|h|m|h|l|m]; B side: [h|m|h|l|h|m], so that
 // segment s of A times segment s of B runs over the six products hh, hm, mh, hl, lh, mm.
 __device__ __forceinline__ void bf16x3_parts(float x, int b_side, __nv_bfloat16* six)
@@ -1243,7 +1243,7 @@ int osb_softmax(const void* x, void* y, int dtype, int64_t rows, int64_t cols, v
     if (rows * cols == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     int threads = cols >= 1024 ? 256 : (cols >= 256 ? 128 : 32);
-    int grid = (int)min<int64_t>(rows, 148 * 16);
+    int grid = (int)min<int64_t>(rows, OSB_SMS * 16);
     if (dtype == OSB_F16) osb_launch((softmax_kernel<__half>), grid, threads, 0, st, (const __half*)x, (__half*)y, rows, cols);
     else if (dtype == OSB_F32) osb_launch((softmax_kernel<float>), grid, threads, 0, st, (const float*)x, (float*)y, rows, cols);
     else return (int)cudaErrorInvalidValue;
@@ -1265,7 +1265,7 @@ int osb_layer_norm(const void* x, void* y, int dtype, int64_t rows, int64_t cols
         return launched();
     }
     int threads = cols >= 1024 ? 256 : (cols >= 256 ? 128 : 32);
-    int grid = (int)min<int64_t>(rows, 148 * 16);
+    int grid = (int)min<int64_t>(rows, OSB_SMS * 16);
     if (dtype == OSB_F16) osb_launch((layer_norm_kernel<__half>), grid, threads, 0, st, (const __half*)x, (__half*)y, rows, cols, (const __half*)gamma, (const __half*)beta, eps);
     else if (dtype == OSB_F32) osb_launch((layer_norm_kernel<float>), grid, threads, 0, st, (const float*)x, (float*)y, rows, cols, (const float*)gamma, (const float*)beta, eps);
     else return (int)cudaErrorInvalidValue;
@@ -1277,7 +1277,7 @@ int osb_reduce_mean(const void* x, void* y, int dtype, int64_t rows, int64_t col
     if (rows * cols == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     int threads = cols >= 1024 ? 256 : (cols >= 256 ? 128 : 32);
-    int grid = (int)min<int64_t>(rows, 148 * 16);
+    int grid = (int)min<int64_t>(rows, OSB_SMS * 16);
     if (dtype == OSB_F16) osb_launch((reduce_mean_kernel<__half>), grid, threads, 0, st, (const __half*)x, (__half*)y, rows, cols);
     else if (dtype == OSB_F32) osb_launch((reduce_mean_kernel<float>), grid, threads, 0, st, (const float*)x, (float*)y, rows, cols);
     else return (int)cudaErrorInvalidValue;
@@ -1288,7 +1288,7 @@ int osb_instance_norm(const void* x, void* y, int dtype, int64_t channels, int64
 {
     if (channels * n_per_c == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    int splits = (int)max<int64_t>(1, min<int64_t>(64, (148 * 4 + channels - 1) / channels));
+    int splits = (int)max<int64_t>(1, min<int64_t>(64, (OSB_SMS * 4 + channels - 1) / channels));
     while (splits > 1 && n_per_c / splits < 1024) splits--;
     while (splits > 1 && (size_t)channels * splits * 2 > OSB_WS_INORM_DOUBLES) splits--;
     if ((size_t)channels * splits * 2 > OSB_WS_INORM_DOUBLES) return (int)cudaErrorInvalidValue;
@@ -1325,7 +1325,7 @@ int osb_group_norm(const void* x, void* y, int dtype, int nhwc, int64_t C, int64
             double* fstats = (double*)((char*)stats_ + 1024);
             int* counters = (int*)((char*)stats_ + 1920);
             // one CTA per SM by default (every CTA must be co-resident for the rendezvous; fewer CTAs = fewer same-address atomics)
-            static const int cta_cap = [] { const char* e = getenv("OSB_GN_CTAS"); int v = e ? atoi(e) : 0; return v > 0 ? v : 148; }();
+            static const int cta_cap = [] { const char* e = getenv("OSB_GN_CTAS"); int v = e ? atoi(e) : 0; return v > 0 ? v : OSB_SMS; }();
             int threads = C / vec <= 256 ? 256 : 512;
             size_t smem = sizeof(float) * 2 * groups;
             // co-residency bound from the device itself (SM count x resident CTAs of THIS kernel at this block size), and a cooperative
@@ -1352,13 +1352,13 @@ int osb_group_norm(const void* x, void* y, int dtype, int nhwc, int64_t C, int64
     if (e != cudaSuccess) return (int)e;
     size_t n = (size_t)C * HW;
     if (nhwc) {
-        int64_t ctas = min<int64_t>(HW, 148 * 4);
+        int64_t ctas = min<int64_t>(HW, OSB_SMS * 4);
         int64_t ppc = (HW + ctas - 1) / ctas;
         ctas = (HW + ppc - 1) / ppc;
         size_t smem = sizeof(float) * 2 * groups;
         int vec = dtype == OSB_F16 ? 8 : 4;
         if (C % vec == 0 && C / vec <= 256 && aligned16(x)) {
-            int64_t c2 = min<int64_t>(HW, 148 * 2);
+            int64_t c2 = min<int64_t>(HW, OSB_SMS * 2);
             int64_t ppc2 = (HW + c2 - 1) / c2;
             c2 = (HW + ppc2 - 1) / ppc2;
             const size_t smem2 = sizeof(float) * (2 * groups + (size_t)(256 / (C / vec)) * 2 * C);    // + the per-row partials
@@ -1373,7 +1373,7 @@ int osb_group_norm(const void* x, void* y, int dtype, int nhwc, int64_t C, int64
         else return (int)cudaErrorInvalidValue;
     } else {
         int64_t n_per_g = (C / groups) * HW;
-        int splits = (int)max<int64_t>(1, min<int64_t>(64, (148 * 4 + groups - 1) / groups));
+        int splits = (int)max<int64_t>(1, min<int64_t>(64, (OSB_SMS * 4 + groups - 1) / groups));
         while (splits > 1 && n_per_g / splits < 2048) splits--;
         dim3 grid((unsigned)groups, (unsigned)splits);
         if (dtype == OSB_F16) osb_launch((gn_stats_nchw_kernel<__half>), grid, 256, 0, st, (const __half*)x, stats, n_per_g, splits);
@@ -1407,7 +1407,7 @@ int osb_group_norm_apply(const void* x, void* y, int dtype, int64_t C, int64_t H
     const size_t smem = sizeof(float) * 2 * (size_t)C;
     const int64_t nvec = HW * (C / vec);
     // every CTA pays the table set-up (C channels, a few hundred cycles); 4 vectors per thread per pass, up to 4 CTAs per SM
-    const int grid = (int)max<int64_t>(1, min<int64_t>((nvec + 256 * 4 - 1) / (256 * 4), 148 * 4));
+    const int grid = (int)max<int64_t>(1, min<int64_t>((nvec + 256 * 4 - 1) / (256 * 4), OSB_SMS * 4));
     if (dtype == OSB_F16) osb_launch((gn_apply_pre_kernel<__half, 8>), grid, 256, smem, st, (const __half*)x, (__half*)y, (const double*)stats, (double*)clear_stats, (int)C, HW, groups, (const __half*)gamma, (const __half*)beta, eps, fuse_silu);
     else if (dtype == OSB_F32) osb_launch((gn_apply_pre_kernel<float, 4>), grid, 256, smem, st, (const float*)x, (float*)y, (const double*)stats, (double*)clear_stats, (int)C, HW, groups, (const float*)gamma, (const float*)beta, eps, fuse_silu);
     else return (int)cudaErrorInvalidValue;
@@ -1426,7 +1426,7 @@ int osb_channel_add_stats(const void* x, const void* addv, void* y, int dtype, i
     // pixels per CTA: enough CTAs to fill the machine (4 per SM), but >= 4 pixel rows per thread-row so the unrolled loop is used;
     // each CTA ends with 2 * groups fp64 atomics, so more CTAs is not free
     const int rows_per_cta = (int)max<int64_t>(1, 256 / (C / vec));
-    int64_t c2 = min<int64_t>((HW + 4 * rows_per_cta - 1) / (4 * rows_per_cta), 148 * 4);
+    int64_t c2 = min<int64_t>((HW + 4 * rows_per_cta - 1) / (4 * rows_per_cta), OSB_SMS * 4);
     c2 = max<int64_t>(c2, 1);
     int64_t ppc2 = (HW + c2 - 1) / c2;
     c2 = (HW + ppc2 - 1) / ppc2;
@@ -1504,7 +1504,7 @@ int osb_softmax_qu8(const void* x, void* y, int64_t rows, int64_t cols, float in
 {
     if (rows * cols == 0) return 0;
     int threads = cols >= 1024 ? 256 : (cols >= 256 ? 128 : 32);
-    osb_launch((softmax_qu8_kernel), (unsigned)min<int64_t>(rows, 148 * 16), threads, 0, (cudaStream_t)stream, (const uint8_t*)x, (uint8_t*)y, rows, cols, in_scale, out_scale, out_zp);
+    osb_launch((softmax_qu8_kernel), (unsigned)min<int64_t>(rows, OSB_SMS * 16), threads, 0, (cudaStream_t)stream, (const uint8_t*)x, (uint8_t*)y, rows, cols, in_scale, out_scale, out_zp);
     return launched();
 }
 
@@ -1512,7 +1512,7 @@ int osb_rms_norm(const void* x, int xd, const void* w, int wd, void* y, int yd, 
 {
     if (rows * cols == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    const unsigned grid = (unsigned)min<int64_t>((rows + 3) / 4, 148 * 8);
+    const unsigned grid = (unsigned)min<int64_t>((rows + 3) / 4, OSB_SMS * 8);
     const bool per_block = rows <= 64 && cols >= 512;
 #define OSB_RMS(TI_, TW_, TO_) do { if (per_block) osb_launch((rms_norm_block_kernel<TI_, TW_, TO_>), (unsigned)rows, 256, 0, st, (const TI_*)x, (const TW_*)w, (TO_*)y, (int)cols, eps); \
                                     else osb_launch((rms_norm_kernel<TI_, TW_, TO_>), grid, 128, 0, st, (const TI_*)x, (const TW_*)w, (TO_*)y, rows, (int)cols, eps); } while (0)
@@ -1544,7 +1544,7 @@ int osb_gather_rows(const void* table, const int64_t* idx, void* out, int64_t n_
 {
     if (n_idx * row_bytes == 0) return 0;
     int threads = row_bytes >= 4096 ? 256 : 64;
-    osb_launch((gather_rows_kernel), (unsigned)min<int64_t>(n_idx, 148 * 8), threads, 0, (cudaStream_t)stream, (const uint8_t*)table, idx, (uint8_t*)out, n_idx, table_rows, row_bytes);
+    osb_launch((gather_rows_kernel), (unsigned)min<int64_t>(n_idx, OSB_SMS * 8), threads, 0, (cudaStream_t)stream, (const uint8_t*)table, idx, (uint8_t*)out, n_idx, table_rows, row_bytes);
     return launched();
 }
 

@@ -1,8 +1,8 @@
 // kernels_gemm.cu -- dispatch for MatMul/Gemm/Conv plus the CUDA-core implicit-GEMM kernels that serve as
 //   (a) the fp32 path (bit-faithful fp32 FMA accumulation, needed for parity with the reference's f32 XNNPACK path),
-//   (b) the fallback for fp16 problems the tcgen05 kernel (gemm_tcgen05.cu) does not take (ragged K, tiny M/N),
+//   (b) the fallback for fp16 problems the tensor-core kernel (gemm_wgmma.cu) does not take (ragged K, tiny M/N),
 //   (c) the qu8 (W8A8) path with XNNPACK's exact requantisation.
-// The tensor-core path for fp16 lives in gemm_tcgen05.cu; osb_gemm/osb_conv2d choose between them.
+// The tensor-core path for fp16 lives in gemm_wgmma.cu; osb_gemm/osb_conv2d choose between them.
 //
 // One kernel template covers GEMM and convolution: a convolution is a GEMM whose A operand is gathered on the fly
 // from the NHWC input (M = Ho*Wo, K = kh*kw*Cin in OHWI order, N = Cout, B = the OHWI weights read as [N, K]).
@@ -11,7 +11,7 @@
 #include "workspace.h"
 #include <cstdlib>
 
-// implemented in gemm_tcgen05.cu
+// implemented in gemm_wgmma.cu
 int osb_tc_gemm_launch(const void* A, const void* B, void* C, const void* bias, const void* residual,
                        int64_t batch, int64_t M, int64_t N, int64_t K, int64_t sa, int64_t sb, int64_t sc,
                        int b_transposed, cudaStream_t st, int64_t lda, int64_t ldb, int64_t ldc);
@@ -222,7 +222,7 @@ __device__ __forceinline__ void gemv_panel_body(const T* __restrict__ A, const T
         for (int v = 0; v < VEC; v++) acc[m][v] = 0.f;
     if (n0 < N) {
         // GEMV_U independent 16-byte loads per thread before the first FMA: a decode GEMV is pure weight streaming and one load in
-        // flight per thread left HBM at ~1 TB/s (ncu, r02_launches_llama.csv); 8 x 16 B x 128 threads x 4 CTAs = 64 KB in flight per SM
+        // flight per thread leaves HBM bandwidth unused; 8 x 16 B x 128 threads x 4 CTAs = 64 KB in flight per SM
         for (int k = k_lo + kl; k < k_hi; k += 4 * GEMV_U) {
             Vec<T, VEC> b[GEMV_U];
 #pragma unroll
@@ -798,7 +798,7 @@ int osb_gemm_ld(const void* A, int64_t lda, const void* B, int64_t ldb, void* C,
         }
     }
     if (dense && M <= 8 && batch == 1) {
-        int grid = bt ? (int)min<int64_t>((N + 7) / 8, 148 * 8) : (int)((N + 63) / 64);
+        int grid = bt ? (int)min<int64_t>((N + 7) / 8, OSB_SMS * 8) : (int)((N + 63) / 64);
         if (dtype == OSB_F16) osb_launch((skinny_gemm_kernel<__half, 8>), grid, 256, 0, st, (const __half*)A, (const __half*)B, (__half*)C, (const __half*)bias, (const __half*)residual, (int)M, (int)N, (int)K, bt);
         else osb_launch((skinny_gemm_kernel<float, 8>), grid, 256, 0, st, (const float*)A, (const float*)B, (float*)C, (const float*)bias, (const float*)residual, (int)M, (int)N, (int)K, bt);
         return launched();
@@ -934,11 +934,11 @@ int osb_softmax_scaled_ld(const void* x, void* y, int dtype, int64_t rows, int64
     if (rows * cols == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     int threads = cols >= 1024 ? 256 : (cols >= 256 ? 128 : 32);
-    int grid = (int)min<int64_t>(rows, 148 * 16);
+    int grid = (int)min<int64_t>(rows, OSB_SMS * 16);
     if (mask_rows <= 0) mask_rows = 1;
     int vecw = dtype == OSB_F16 ? 8 : 4;
     if (ld <= 256 && cols <= ld) {
-        grid = (int)min<int64_t>((rows + 7) / 8, 148 * 8);
+        grid = (int)min<int64_t>((rows + 7) / 8, OSB_SMS * 8);
         if (dtype == OSB_F16) osb_launch((softmax_scaled_warp_kernel<__half>), grid, 256, 0, st, (const __half*)x, (__half*)y, rows, (int)cols, (int)ld, scale, (const __half*)mask, mask_rows);
         else if (dtype == OSB_F32) osb_launch((softmax_scaled_warp_kernel<float>), grid, 256, 0, st, (const float*)x, (float*)y, rows, (int)cols, (int)ld, scale, (const float*)mask, mask_rows);
         else return (int)cudaErrorInvalidValue;
@@ -947,7 +947,7 @@ int osb_softmax_scaled_ld(const void* x, void* y, int dtype, int64_t rows, int64
     if (ld != cols) return (int)cudaErrorInvalidValue;   // padded rows are only needed (and supported) for short rows
     if (cols >= 512 && cols <= 12288 && cols % vecw == 0 && aligned16(x) && aligned16(y)) {
         size_t smem = (size_t)cols * sizeof(float);
-        grid = (int)min<int64_t>(rows, 148 * 4);
+        grid = (int)min<int64_t>(rows, OSB_SMS * 4);
         if (dtype == OSB_F16) {
             static bool attr16 = false;
             if (!attr16) { cudaFuncSetAttribute(softmax_scaled_smem_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 12288 * 4); attr16 = true; }
@@ -990,7 +990,7 @@ int osb_attention(const void* q, const void* k, const void* v, const void* mask,
     int warps = 4;
     size_t smem = (size_t)warps * (d + dv + 32) * sizeof(float);
     if (smem > 48 * 1024) return (int)cudaErrorInvalidValue;
-    int grid = (int)min<int64_t>((heads * Tq + warps - 1) / warps, 148 * 8);
+    int grid = (int)min<int64_t>((heads * Tq + warps - 1) / warps, OSB_SMS * 8);
     if (dtype == OSB_F16) osb_launch((attention_rows_kernel<__half>), grid, warps * 32, smem, st, (const __half*)q, (const __half*)k, (const __half*)v, (const __half*)mask, (__half*)out, heads, Tq, Tk, (int)d, (int)dv, scale, k_transposed, kv_group);
     else if (dtype == OSB_F32) osb_launch((attention_rows_kernel<float>), grid, warps * 32, smem, st, (const float*)q, (const float*)k, (const float*)v, (const float*)mask, (float*)out, heads, Tq, Tk, (int)d, (int)dv, scale, k_transposed, kv_group);
     else return (int)cudaErrorInvalidValue;
@@ -1001,7 +1001,7 @@ int osb_attention(const void* q, const void* k, const void* v, const void* mask,
 static int g_pdl = -1;
 int osb_pdl_enabled(void)
 {
-    // measured on B200: inside a CUDA graph PDL costs ~7% on this workload, so it is opt-in (OSB_PDL=1)
+    // opt-in (OSB_PDL=1): inside a CUDA graph PDL did not pay on this workload
     if (g_pdl < 0) { const char* e = getenv("OSB_PDL"); g_pdl = (e && e[0] == '1') ? 1 : 0; }
     return g_pdl;
 }

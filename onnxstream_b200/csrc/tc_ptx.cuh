@@ -1,4 +1,5 @@
-// tc_ptx.cuh -- inline-PTX wrappers shared by the tcgen05 kernels (gemm_tcgen05.cu: one CTA per tile; gemm2_tcgen05.cu: CTA pairs).
+// tc_ptx.cuh -- inline-PTX wrappers shared by the sm_90a tensor-core kernels (gemm_wgmma.cu, attention_wgmma.cu): mbarrier, TMA,
+// shared-memory matrix descriptors and warpgroup MMA (wgmma).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -35,32 +36,50 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
             "selp.u32 %0, 1, 0, p;\n\t"
             "}" : "=r"(done) : "r"(addr), "r"(parity) : "memory");
         if (done) break;
-        // watchdog: a protocol bug must surface as a launch failure, never as a hung GPU (~2 s at 2 GHz)
+        // watchdog: a protocol bug must surface as a launch failure, never as a hung GPU (~2 s at 2 GHz).  No printf here: a function
+        // call inside the MMA loop makes ptxas serialise every wgmma.
         long long now = clock64();
         if (t0 == 0) t0 = now;
-        else if (now - t0 > 4000000000LL) { printf("tcgen05 kernel: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
+        else if (now - t0 > 4000000000LL) __trap();
     }
 }
 
-__device__ __forceinline__ void tma_load_2d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1)
-{
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(smem)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2)
 {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_u32(smem)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-
-// The producer / MMA warps run WARP-UNIFORM control flow and issue from an elect.sync-guarded region.  (Inside an
-// `if (lane == 0)` region ptxas cannot keep the operands of UTCHMMA / UTMALDG in uniform registers and wraps every one of them
-// in an ELECT + R2UR.BROADCAST + BRA.U.ANY loop: ~1000 issue cycles per k-block, measured with ncu source sampling.)
+// The producer warp runs WARP-UNIFORM control flow and issues from an elect.sync-guarded region, so ptxas keeps the TMA operands in
+// uniform registers.
 __device__ __forceinline__ void tma_load_3d_s(uint32_t smem_addr, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2)
 {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_addr), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
+// TMA multicast: the box lands at the same shared-memory offset in every CTA of `cta_mask` and completes bytes on the mbarrier at the
+// same offset in each of them
+__device__ __forceinline__ void tma_load_3d_mc(uint32_t smem_addr, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, uint16_t cta_mask)
+{
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;"
+                 ::"r"(smem_addr), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask) : "memory");
+}
+
+// ---- thread-block clusters ----
+__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ uint32_t cluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
+__device__ __forceinline__ uint32_t cluster_count_x() { uint32_t r; asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r)); return r; }
+// every thread of every CTA of the cluster; orders shared-memory writes (barrier init) before the peers use them
+__device__ __forceinline__ void cluster_sync()
+{
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta)
+{
+    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\tmbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+                 ::"r"(smem_u32(bar)), "r"(cta) : "memory");
+}
+
 // one lane of a converged warp, chosen by the hardware (elect.sync): ptxas knows the guarded region runs on exactly one lane
 __device__ __forceinline__ bool elect_one()
 {
@@ -69,96 +88,91 @@ __device__ __forceinline__ bool elect_one()
     return pred != 0;
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], single CTA, fp16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier once all previously issued MMAs have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// shared-memory matrix descriptor (see cute/arch/mma_sm100_desc.hpp SmemDescriptor): SWIZZLE_128B, version 1
+// shared-memory matrix descriptor for wgmma (cute/arch/mma_sm90_desc.hpp GmmaDescriptor): 128B swizzle, start / LBO / SBO in 16-byte units.
+//   K-major: 8-row groups SBO bytes apart (LBO unused).  MN-major: 64-element MN atoms LBO bytes apart, 8-row K groups SBO bytes apart.
+// Every operand tile starts on a 1024-byte boundary, so the base-offset field stays 0; advancing K inside a swizzle row adds to the start address.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes)
 {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;   // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;   // LayoutType::SWIZZLE_128B
+    d |= (uint64_t)1 << 62;   // layout type SWIZZLE_128B
     return d;
+}
+
+// wgmma ordering: fence before the first MMA that reads registers written by ordinary code, commit the issued MMAs as one group, and
+// wait until at most N groups are still in flight
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// Accumulator fragments of an m64nN wgmma: thread t of the warpgroup holds, for every 8-column block j, d[4j], d[4j+1] at row
+// 16 (t / 32) + (t % 32) / 4, columns 8j + 2 (t % 4) + {0, 1}, and d[4j+2], d[4j+3] at the row 8 below.
+template <int TRANS_B>
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, %67;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
+}
+template <int TRANS_B>
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, %67;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
+}
+__device__ __forceinline__ void wgmma_m64n128k32_u8(int32_t (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_m64n64k16_f16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
 }
 
 
 // ---- GroupNorm statistics of a GEMM / conv output, gathered in the producing kernel's epilogue -----------------------------------
-// The consumer GroupNorm needs sum(x) and sum(x^2) per group of `cpg` consecutive channels over ALL rows (pixels).  In the epilogue a
-// lane owns one ROW of the tile (TMEM lane = row), so per-column sums need a transpose: the warp parks its 32 x 32 chunk of fp16-rounded
-// outputs in a private 2 KiB shared buffer (row pitch 64 B, 16-byte units XOR-swizzled by (row >> 1) & 3: conflict-free writes), then lane
-// l walks column l down the 32 rows (one wavefront per row), and adds its column's (sum, sum of squares) to the CTA's per-group
-// shared accumulators.  After the tile the accumulators are flushed to the global fp64 statistics (the reference accumulates in double,
-// src/onnxstream.cpp:4788-5055) -- fp32 only ever sums <= 128 rows x cpg values.
+// The consumer GroupNorm needs sum(x) and sum(x^2) per group of `cpg` consecutive channels over ALL rows (pixels).  A thread holds two
+// adjacent columns of two rows per 8-column block (the accumulator fragment above): the 8 lanes that share those columns sum their rows by
+// shuffle, and lanes 0..3 add the column totals to the CTA's per-group shared accumulators.  After the tile the accumulators are flushed to
+// the global fp64 statistics (the reference accumulates in double) -- fp32 only ever sums <= 128 rows x cpg values.
 constexpr int GN_MAX_GROUPS = 64;
 
-// h: this lane's row, 32 fp16 values already rounded as they are stored (rows outside the problem must be passed as zeros)
-__device__ __forceinline__ void gn_stats_chunk(uint32_t wbuf, const uint32_t (&h)[16], int n_base, int n_end, int cpg, float* cta_stats, int lane)
+// v0 / v1: this thread's two columns (n, n + 1), each summed over its two rows, values already rounded as they are stored (rows outside
+// the problem passed as zeros); q0 / q1 the same for the squares
+__device__ __forceinline__ void gn_stats_pair(float v0, float v1, float q0, float q1, int n, int n_end, int cpg, float* cta_stats, int lane)
 {
-    const uint32_t row = wbuf + (uint32_t)lane * 64u;
-    const uint32_t sw = ((uint32_t)lane >> 1) & 3u;
 #pragma unroll
-    for (uint32_t u = 0; u < 4; u++)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row + ((u ^ sw) << 4)), "r"(h[4 * u]), "r"(h[4 * u + 1]), "r"(h[4 * u + 2]), "r"(h[4 * u + 3]) : "memory");
-    __syncwarp();
-    float s = 0.f, ss = 0.f;
-    const uint32_t unit = (uint32_t)lane >> 3, within = ((uint32_t)lane & 7u) * 2u;
-#pragma unroll
-    for (uint32_t r = 0; r < 32; r++) {
-        unsigned short raw;
-        asm volatile("ld.shared.u16 %0, [%1];" : "=h"(raw) : "r"(wbuf + r * 64u + ((unit ^ ((r >> 1) & 3u)) << 4) + within));
-        const float v = __half2float(__ushort_as_half(raw));
-        s += v; ss = fmaf(v, v, ss);
+    for (int off = 4; off < 32; off <<= 1) {
+        v0 += __shfl_xor_sync(0xffffffffu, v0, off); v1 += __shfl_xor_sync(0xffffffffu, v1, off);
+        q0 += __shfl_xor_sync(0xffffffffu, q0, off); q1 += __shfl_xor_sync(0xffffffffu, q1, off);
     }
-    // lane l holds column n_base + l; the lanes of one group are contiguous: segmented suffix sums by shuffle (5 steps) leave each
-    // group's total in its first lane, which alone touches the shared accumulator -- 32 colliding float atomics per chunk measured
-    // +10 us per launch (profiles/r02_ab_epilogue.txt)
-    const int n = n_base + lane;
-    const int g = n / cpg;
-    if (n >= n_end) { s = 0.f; ss = 0.f; }
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        const float ts = __shfl_down_sync(0xffffffffu, s, off), tss = __shfl_down_sync(0xffffffffu, ss, off);
-        if (lane + off < 32 && (n + off) / cpg == g) { s += ts; ss += tss; }
+    if (lane < 4 && n < n_end) {
+        const int g0 = n / cpg;
+        if (n + 1 < n_end && (n + 1) / cpg == g0) { v0 += v1; q0 += q1; }
+        else if (n + 1 < n_end) { atomicAdd(&cta_stats[2 * (g0 + 1)], v1); atomicAdd(&cta_stats[2 * (g0 + 1) + 1], q1); }
+        atomicAdd(&cta_stats[2 * g0], v0);
+        atomicAdd(&cta_stats[2 * g0 + 1], q0);
     }
-    const bool head = lane == 0 || (n - 1) / cpg != g;
-    if (head && n < n_end) {
-        atomicAdd(&cta_stats[2 * g], s);
-        atomicAdd(&cta_stats[2 * g + 1], ss);
-    }
-    __syncwarp();
 }
 
 // after a tile: thread t of the epilogue group moves accumulator t to the global fp64 statistics and re-arms it

@@ -1,7 +1,7 @@
 """Host-side Python mirror of OnnxStream's FFI surface (reference: src/exports.cpp:42-311, src/bindings.py).
 
 `Model` drives any shared library that exports the 16 ``model_*`` C entry points declared in
-``include/onnxstream_b200.h`` -- the B200 engine (``onnxstream_b200/csrc/libonnxstream_b200.so``) by default; the
+``include/onnxstream_b200.h`` -- the engine (``onnxstream_b200/csrc/libonnxstream_b200.so``) by default; the
 test-suite points the same class at the reference compiled in place, so both sides of a parity test are driven
 identically.  This module never loads a checker library on its own.  Method names,
 argument meaning and error behaviour follow the reference's ``bindings.py`` so parity tests read the same on
@@ -89,7 +89,7 @@ def load_library(path: str) -> ctypes.CDLL:
 
 def plan_summary(model_text: str, fp16_arithmetic: bool = True, fuse_nodes: bool = True, fuse_attention: bool = True,
                  use_scaled_dp_attn_op: bool = False, library_path: Optional[str] = None) -> str:
-    """B200 engine only, needs no GPU: the fusion plan for `model_text` -- one line per execution step
+    """Engine only, needs no GPU: the fusion plan for `model_text` -- one line per execution step
     ("KIND n_ops first_op_type first_op_name") and a final "#summary" line (include/onnxstream_b200.h)."""
     lib = load_library(library_path or ENGINE_LIB)
     p = lib.model_b200_plan_summary(model_text.encode(), int(fp16_arithmetic), int(fuse_nodes), int(fuse_attention), int(use_scaled_dp_attn_op))
@@ -189,7 +189,7 @@ class Model:
         ctypes.memmove(ptr, array.ctypes.data, array.nbytes)
 
     def get_tensor(self, name: str, index: int = 0) -> Optional[np.ndarray]:
-        """index > 0 (B200 engine only): the index-th batch sibling pushed / produced under `name`."""
+        """index > 0 (engine only): the index-th batch sibling pushed / produced under `name`."""
         ptr = self.lib.model_get_tensor(self.h, name.encode()) if index == 0 else self.lib.model_ext_get_tensor_at(self.h, name.encode(), index)
         if not ptr:
             return None
@@ -237,14 +237,14 @@ class Model:
                    "tc_launches", "steps_executed", "ops_fused_away", "last_run_ms", "last_gpu_ms", "graph_replays", "side_steps")
 
     def run_resident(self, steps: int) -> float:
-        """B200 engine only: replay the captured CUDA graph `steps` times on device-resident inputs; returns CUDA-event ms."""
+        """Engine only: replay the captured CUDA graph `steps` times on device-resident inputs; returns CUDA-event ms."""
         ms = self.lib.model_b200_run_resident(self.h, steps)
         if ms < 0:
             raise OnnxStreamError("model_b200_run_resident failed (no captured graph?)")
         return ms
 
     def stats(self) -> Dict[str, float]:
-        """B200 engine only: streaming / launch statistics of the last run (include/onnxstream_b200.h)."""
+        """Engine only: streaming / launch statistics of the last run (include/onnxstream_b200.h)."""
         out = (ctypes.c_double * len(self.STAT_FIELDS))()
         self.lib.model_b200_get_stats(self.h, out, len(self.STAT_FIELDS))
         return dict(zip(self.STAT_FIELDS, list(out)))

@@ -1,5 +1,5 @@
 """Generates the golden vectors in this directory from oracle/_ref (the reference's own sources compiled in place).
-Run here (needs /root/reference for the oracle build):  python tests/golden/make_golden.py
+Needs the oracle build (__graft_entry__.build() with a reference checkout available):  python tests/golden/make_golden.py
 Each case = a seeded synthetic model directory (rebuilt deterministically by `build_case`) + inputs -> the reference output."""
 import os
 import sys

@@ -64,8 +64,8 @@ GEMM_CASES = [
 
 
 PAIR_GEMM_CASES = [
-    # the CTA-pair kernel (cta_group::2, 256 x bn tiles, TMA-store epilogue) forced on: both B majors, ragged M / N / K, odd number
-    # of 128-row tiles (the pair's second half is empty), batch, bias / residual, every tile width
+    # CTA pairs (2-CTA clusters sharing the B tile through TMA multicast) forced on: both B majors, ragged M / N / K, odd number
+    # of 128-row tiles (the pair's second tile is empty), batch, bias / residual
     (1, 256, 256, 128, 1, False, False),
     (1, 256, 256, 128, 0, False, False),
     (1, 300, 136, 72, 1, True, True),
@@ -78,7 +78,7 @@ PAIR_GEMM_CASES = [
     (1, 2048, 640, 5760, 1, True, False),
     (3, 520, 264, 136, 1, False, True),
     (2, 512, 512, 256, 0, True, False),
-    (1, 8192, 1024, 512, 1, False, False),    # several tiles per pair: accumulator double buffering, staging reuse across tiles
+    (1, 8192, 1024, 512, 1, False, False),    # several tiles per pair: ring reuse across tiles
 ]
 
 
@@ -94,7 +94,7 @@ def test_gemm_f16_pair_kernel(K, case):
 PAIR_CONV_CASES = [
     (64, 64, 320, 320, 3, 1, 1, True, True),
     (32, 32, 96, 72, 3, 1, 1, False, False),      # ragged channels
-    (24, 40, 32, 40, 3, 1, 1, True, False),       # non power-of-two width: boxes clipped by the store
+    (24, 40, 32, 40, 3, 1, 1, True, False),       # non power-of-two width
     (256, 256, 32, 16, 3, 1, 1, True, False),     # wide image: bw = 128, one row segment per CTA
     (16, 16, 64, 64, 3, 2, 1, True, False),       # strided
     (64, 64, 320, 320, 3, 2, 1, True, False),
@@ -202,7 +202,7 @@ def test_conv_f16(K, case, impl):
 GN_CONV_CASES = [
     # H, W, Cin, Cout, k, stride, groups, residual, bias2, pair_mode
     (64, 64, 320, 320, 3, 1, 32, True, False, 1),     # cpg = 10: groups straddle 32-column chunks and 128-column tiles
-    (64, 64, 320, 320, 3, 1, 32, False, True, 2),     # same through the CTA-pair kernel, with the time-embedding addend
+    (64, 64, 320, 320, 3, 1, 32, False, True, 2),     # same through CTA pairs, with the time-embedding addend
     (32, 32, 320, 640, 3, 1, 32, False, True, 1),
     (32, 32, 640, 640, 1, 1, 32, True, False, 2),
     (16, 16, 1280, 1280, 3, 1, 32, True, False, 1),   # split-K: statistics in the reduce kernel (cpg = 40)
@@ -216,7 +216,7 @@ GN_CONV_CASES = [
 @pytest.mark.parametrize("case", GN_CONV_CASES)
 def test_conv_epilogue_gn_stats_and_bias2(K, case):
     """osb_conv2d_ex: conv + bias + bias2 (per-channel addend) + residual, with the GroupNorm statistics of the STORED fp16 output
-    gathered in the epilogue (tile epilogue, CTA-pair epilogue or split-K reduce kernel) -- then osb_group_norm_apply on them
+    gathered in the epilogue (single-CTA or CTA-pair tile epilogue, or the split-K reduce kernel) -- then osb_group_norm_apply on them
     against a float64 GroupNorm of the same tensor."""
     import torch
     import torch.nn.functional as Fn
@@ -352,7 +352,7 @@ QU8_TC_GEMM = [(200, 144, 320, 0), (200, 144, 320, 1), (4096, 320, 320, 0), (102
 
 @pytest.mark.parametrize("M,N,Kd,bt", QU8_TC_GEMM)
 def test_qu8_tensor_core_gemm_bit_exact(K, M, N, Kd, bt):
-    """tcgen05.mma.kind::i8 on raw uint8 bytes + zero-point terms from row / column sums + XNNPACK's fp32 requantisation: bit-exact
+    """wgmma .u8 on raw uint8 bytes + zero-point terms from row / column sums + XNNPACK's fp32 requantisation: bit-exact
     against the integer restatement (the one tests/test_cpu.py and the model-level chain test pin to the reference's XNNPACK run).
     Both weight layouts: [K,N] (ONNX MatMul, MN-major B operand) and [N,K]."""
     import torch
@@ -462,7 +462,7 @@ def test_gemm_head_views(K, impl, T, Tk, h, d):
 
 @pytest.mark.parametrize("T,Tk,h,d", [(128, 128, 1, 64), (256, 384, 2, 40), (200, 77, 4, 40), (64, 30, 2, 32), (300, 200, 3, 64), (4096, 4096, 8, 40), (1024, 1024, 10, 64)])
 def test_flash_attention(K, T, Tk, h, d):
-    """Fused tcgen05 attention against softmax(QK^T s)V in fp64 on the fp16-rounded operands.  Tolerance: P is rounded to
+    """Fused wgmma attention against softmax(QK^T s)V in fp64 on the fp16-rounded operands.  Tolerance: P is rounded to
     fp16 before the second MMA (as the reference's fp16 softmax output is), so |err| <= 2^-9 * sum|p_i v_i| + 2^-10 |ref|."""
     import torch
     vp, i64, cf = ctypes.c_void_p, ctypes.c_int64, ctypes.c_float
@@ -541,7 +541,7 @@ def test_group_norm_nhwc(K, dtype, C, HW, silu):
 
 @pytest.mark.parametrize("groups,M,N,Kd", [(3, 4096, 320, 320), (3, 1024, 640, 640), (2, 77, 1280, 768), (3, 256, 1280, 1280), (2, 64, 1280, 1280), (3, 200, 136, 72)])
 def test_gemm_grouped(K, groups, M, N, Kd):
-    """q/k/v projections as one grouped tcgen05 launch: every member must equal its stand-alone GEMM reference."""
+    """q/k/v projections as one grouped tensor-core launch: every member must equal its stand-alone GEMM reference."""
     import torch
     torch.manual_seed(M + N + Kd)
     a = torch.randn(M, Kd, device="cuda").half()
@@ -556,7 +556,7 @@ def test_gemm_grouped(K, groups, M, N, Kd):
     torch.cuda.synchronize()
     assert rc == 0
     if N % 8 == 0 and Kd % 8 == 0 and M >= 32:
-        assert K.osb_tc_launch_count() == 1, "expected ONE tcgen05 launch for the whole group"
+        assert K.osb_tc_launch_count() == 1, "expected ONE tensor-core launch for the whole group"
     for g in range(groups):
         ref = a.double() @ bs[g].double()
         absref = a.double().abs() @ bs[g].double().abs()
@@ -747,7 +747,7 @@ F32X_GEMM = [(77, 768, 768), (77, 3072, 768), (77, 768, 3072), (4096, 320, 320),
 
 @pytest.mark.parametrize("M,N,Kd", F32X_GEMM)
 def test_f32_gemm_on_tensor_cores_bf16_triple_split(K, M, N, Kd):
-    """fp32 MatMul through tcgen05 (bf16 triple split, six cross products in one contraction): as accurate as an fp32 FMA loop.
+    """fp32 MatMul through the tensor cores (bf16 triple split, six cross products in one contraction): as accurate as an fp32 FMA loop.
     Bar: |err| <= 1e-5 * sum|a_i b_i| over every output (a sequential fp32 FMA loop is bounded by K * 2^-24 = 2e-5 at K = 320; the tensor core
     aligns each group of products to the largest one before adding) -- three orders of magnitude below what a single bf16 or tf32 pass gives."""
     import torch
