@@ -142,7 +142,8 @@ int osb_conv2d_fusable(const void* x, const void* w, const void* y, int64_t H, i
 /* RMSNorm y = w * x / sqrt(mean(x^2) + eps) over the last axis, fp32 arithmetic, any mix of fp16 / fp32 storage (the 7-op chain Pow,
  * ReduceMean, Add, Sqrt, Div, Mul, Mul of llm.cpp's graphs; the reference keeps it in fp32 through m_requires_upcast, src/llm.cpp:385-389) */
 int osb_rms_norm(const void* x, int xd, const void* w, int wd, void* y, int yd, int64_t rows, int64_t cols, float eps, void* stream);
-/* rotary embedding, rotate_half form (Slice, Slice, Neg, Concat, Mul, Mul, Add): y = x * cos + rotate_half(x) * sin; cos / sin: 1 or `rows` rows of D */
+/* rotary embedding, rotate_half form (Slice, Slice, Neg, Concat, Mul, Mul, Add): y = x * cos + rotate_half(x) * sin; cos / sin:
+ * `table_rows` rows of D, x row r reads table row r % table_rows (1: one row for every x row; T: x [heads, T, D]) */
 int osb_rope(const void* x, const void* cs, const void* sn, void* y, int dtype, int64_t rows, int64_t D, int64_t table_rows, void* stream);
 /* Decode GEMV with uint8 weights [K,N] dequantised in registers (M <= 2): y = x . ((Wq - zp) * scale rounded to `dtype`) + bias + residual.
  * The uint8-weight / float-arithmetic MatMul of the reference (weights converted at load, src/onnxstream.cpp:2885-2890) at half the HBM bytes. */
@@ -197,6 +198,14 @@ int osb_attention(const void* q, const void* k, const void* v, const void* mask,
 int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype);
 int osb_flash_attention(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
                         int64_t heads, int64_t T, int64_t Tk, int64_t d, float scale, void* stream);
+
+/* Fused flash-style ScaledDotProductAttention on wgmma (fp16; d % 8 == 0, 8 <= d <= 128, dv == d): the prefill case of
+ * src/onnxstream.cpp:7767-7882.  Semantics of osb_attention with k_transposed = 0: q [Hq,Tq,d], k / v [Hkv,Tk,d], additive mask
+ * [Tq,Tk] (optional), out [Hq,Tq,d]; query head h reads KV head h / (Hq / Hkv).  The Hq / Hkv query heads of one KV head are
+ * processed as one [G*Tq, d] row block, so each K / V tile loaded serves all of them.  Any Tq >= 1, Tk >= 1. */
+int osb_sdpa_flash_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, int dtype);
+int osb_sdpa_flash(const void* q, const void* k, const void* v, const void* mask, void* out,
+                   int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, float scale, void* stream);
 
 /* qu8 GEMM / conv with XNNPACK's requantisation (bit-exact target; SURVEY section 8c):
  * acc = sum (x - zx)(w - zw) + bias_i32; y = clamp(lrintf(acc * (sx*sw/sy)) + zy, 0, 255). */

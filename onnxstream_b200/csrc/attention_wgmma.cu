@@ -10,6 +10,9 @@
 //                    (wgmma m64n64k16, V from shared memory), finally O / sum -> fp16 -> global
 // Q, K, V are read in place from the [T, heads*d] projection buffers through strided tensor maps and O is written in the
 // merged [T, heads*d] layout, so the exported graph's head split / merge costs nothing.  d <= 64, d % 8 == 0.
+//
+// sdpa_flash_kernel (below): the same structure for ScaledDotProductAttention with grouped KV heads and an additive mask -- llm.cpp's
+// prompt prefill -- for d <= 128.
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -236,6 +239,268 @@ bool head_map(CUtensorMap* map, const void* base, int d, int heads, int64_t rows
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// ---- grouped-KV masked attention (ScaledDotProductAttention: prompt prefill) ----------------------------------------------------------
+// softmax(Q K^T * scale + mask) V with Hq / Hkv = G query heads per KV head.  The G heads of one KV head are contiguous in q
+// ([G*Tq, d] rows) and in out, so one CTA takes 128 of those packed rows: each K / V tile it loads serves all G heads.  Packed row R
+// is query t = R % Tq of head hk*G + R / Tq and reads mask row t.
+// Same roles as flash_attention_kernel (one TMA producer warp, two consumer warpgroups of 64 rows, K / V ring).  NCH = 64-column
+// chunks of the head dim (1: d <= 64, 2: 64 < d <= 128), BK = keys per tile.  At d = 128 the O accumulator is 64 fp32 registers per
+// thread, so that instantiation takes 64-key tiles (a 32-register score tile) to stay inside the 168 registers of a 384-thread CTA.
+// Masked keys keep their finite logit s*scale + mask (a row whose keys are all masked gets the softmax of those logits, as the
+// reference computes it); keys past Tk are padding (zero-filled by TMA) and get probability 0.
+template <int NCH, int BK>
+struct SdpaCfg {
+    static constexpr int Q_CHUNK = BQ * 128;            // 128 rows x 64 fp16 columns (one 128-byte swizzle row each)
+    static constexpr int KV_CHUNK = BK * 128;
+    static constexpr int Q_BYTES = NCH * Q_CHUNK;
+    static constexpr int KV_BYTES = NCH * KV_CHUNK;     // one K (or V) tile
+    static constexpr int SMEM = Q_BYTES + KV_STAGES * 2 * KV_BYTES + 1024 + 256;
+};
+
+struct SdpaParams {
+    int rows;                // G * Tq: packed query rows per KV head
+    int Tq, Tk, d;
+    int kv_tiles;
+    float scale_log2;        // scale * log2(e)
+    const __half* mask;      // [Tq, Tk] additive, or nullptr
+    __half* out;             // [Hkv][G*Tq][d] (= [Hq, Tq, d])
+};
+
+// mask[row][col], mask[row][col + 1] as a packed half2; keys past Tk read as 0 (they are set to -inf afterwards).  vec: the pair is
+// 4-byte aligned (Tk even).
+__device__ __forceinline__ uint32_t ld_mask_pair(const __half* row, int col, int Tk, bool vec)
+{
+    const unsigned short* m = reinterpret_cast<const unsigned short*>(row) + col;
+    if (col + 1 < Tk) {
+        if (vec) return __ldg(reinterpret_cast<const unsigned int*>(m));
+        return (uint32_t)__ldg(m) | ((uint32_t)__ldg(m + 1) << 16);
+    }
+    return col < Tk ? (uint32_t)__ldg(m) : 0u;
+}
+
+template <int BK>
+__device__ __forceinline__ void qk_mma(float (&s)[BK / 2], uint64_t da, uint64_t db)
+{
+    if constexpr (BK == 128) wgmma_m64n128k16_f16<0>(s, da, db, 1u);
+    else wgmma_m64n64k16_f16<0>(s, da, db, 1u);
+}
+
+template <int NCH, int BK>
+__global__ void __launch_bounds__(FA_THREADS, 1)
+sdpa_flash_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+                  const SdpaParams p)
+{
+    using C = SdpaCfg<NCH, BK>;
+    constexpr float LOG2E = 1.4426950408889634f;
+    osb_pdl_trigger_entry();
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint8_t* sQ = smem;
+    uint8_t* sK = sQ + C::Q_BYTES;
+    uint8_t* sV = sK + KV_STAGES * C::KV_BYTES;
+    uint64_t* bars = (uint64_t*)(sV + KV_STAGES * C::KV_BYTES);
+    uint64_t* q_full = bars;                           // [1]
+    uint64_t* kv_full = bars + 1;                      // [KV_STAGES]
+    uint64_t* kv_empty = kv_full + KV_STAGES;          // [KV_STAGES]
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int r0 = blockIdx.x * BQ, hk = blockIdx.y;
+
+    if (warp == 0 && lane == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
+    }
+    if (warp == 1 && lane == 0) {
+        mbar_init(q_full, 1);
+        for (int i = 0; i < KV_STAGES; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], FA_CONSUMERS); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    osb_pdl_wait();
+
+    const int n_kv = p.kv_tiles;
+
+    if (warp == 0) {
+        if (elect_one()) {
+            mbar_expect_tx(q_full, C::Q_BYTES);
+#pragma unroll
+            for (int c = 0; c < NCH; c++) tma_load_3d(sQ + c * C::Q_CHUNK, &map_q, q_full, 64 * c, r0, hk);
+        }
+        __syncwarp();
+        for (int j = 0; j < n_kv; j++) {
+            const int st = j % KV_STAGES;
+            mbar_wait(&kv_empty[st], ((j / KV_STAGES) & 1) ^ 1);
+            if (elect_one()) {
+                mbar_expect_tx(&kv_full[st], 2 * C::KV_BYTES);
+#pragma unroll
+                for (int c = 0; c < NCH; c++) {
+                    tma_load_3d(sK + st * C::KV_BYTES + c * C::KV_CHUNK, &map_k, &kv_full[st], 64 * c, j * BK, hk);
+                    tma_load_3d(sV + st * C::KV_BYTES + c * C::KV_CHUNK, &map_v, &kv_full[st], 64 * c, j * BK, hk);
+                }
+            }
+            __syncwarp();
+        }
+        osb_pdl_trigger_late();
+    } else if (warp >= 4) {
+        // Fragments as in flash_attention_kernel: rows r, r + 8 of the warpgroup's 64; per 8-column block c the columns 8c + cq, + 1.
+        const int wg = (warp >> 2) - 1;
+        const int r = (warp & 3) * 16 + (lane >> 2);
+        const int cq = 2 * (lane & 3);
+        // Q / K K-major (one descriptor per 64-column chunk, 32 B per 16-element K step); V MN-major, 16 keys = 2048 B per K step
+        const uint64_t qdesc = make_smem_desc(smem_u32(sQ) + wg * (BQ / 2) * 128, 16, 1024);
+        const uint64_t kdesc0 = make_smem_desc(smem_u32(sK), 16, 1024);
+        const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), C::KV_CHUNK, 1024);
+        const bool has_mask = p.mask != nullptr, vec = (p.Tk & 1) == 0;
+        const __half* mrow[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int R = r0 + wg * (BQ / 2) + r + 8 * h;                     // rows past G*Tq (zero-filled by TMA) are never stored
+            mrow[h] = has_mask ? p.mask + (long long)(R % p.Tq) * p.Tk : nullptr;
+        }
+        float o[NCH][32];
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+            for (int i = 0; i < 32; i++) o[ch][i] = 0.f;
+        float m_run[2] = { -INFINITY, -INFINITY }, l_run[2] = { 0.f, 0.f };
+        mbar_wait(q_full, 0);
+        for (int j = 0; j < n_kv; j++) {
+            const int ks = j % KV_STAGES;
+            const int key0 = j * BK;
+            mbar_wait(&kv_full[ks], (j / KV_STAGES) & 1);
+            float s[BK / 2];
+#pragma unroll
+            for (int i = 0; i < BK / 2; i++) s[i] = 0.f;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < NCH * 4; k++)
+                qk_mma<BK>(s, qdesc + (uint64_t)(((k >> 2) * C::Q_CHUNK >> 4) + (k & 3) * 2),
+                           kdesc0 + (uint64_t)((ks * C::KV_BYTES + (k >> 2) * C::KV_CHUNK) >> 4) + (uint64_t)((k & 3) * 2));
+            wgmma_commit();
+            // the mask loads (L2-resident: every head reads the same [Tq, Tk] block) are in flight while the MMAs run
+            uint32_t mk[2][BK / 8];
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int c = 0; c < BK / 8; c++) mk[h][c] = has_mask ? ld_mask_pair(mrow[h], key0 + 8 * c + cq, p.Tk, vec) : 0u;
+            wgmma_wait<0>();
+            // logits in log2 units: s * scale * log2e + mask * log2e; padding keys (last tile only) -inf
+            const bool tail = key0 + BK > p.Tk;
+#pragma unroll
+            for (int c = 0; c < BK / 8; c++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    __half2 m2 = *reinterpret_cast<__half2*>(&mk[h][c]);
+                    const float2 mf = __half22float2(m2);
+                    float x0 = fmaf(s[4 * c + 2 * h], p.scale_log2, mf.x * LOG2E);
+                    float x1 = fmaf(s[4 * c + 2 * h + 1], p.scale_log2, mf.y * LOG2E);
+                    if (tail) {
+                        if (key0 + 8 * c + cq >= p.Tk) x0 = -INFINITY;
+                        if (key0 + 8 * c + cq + 1 >= p.Tk) x1 = -INFINITY;
+                    }
+                    s[4 * c + 2 * h] = x0; s[4 * c + 2 * h + 1] = x1;
+                }
+            float alpha[2], neg_m[2];
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                float mt = -INFINITY;
+#pragma unroll
+                for (int c = 0; c < BK / 8; c++) mt = fmaxf(mt, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
+                mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+                mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+                const float m_new = fmaxf(m_run[h], mt);
+                // m_new = -inf only when every logit so far is -inf (a -inf mask): keep the sums at 0 instead of producing NaN here
+                const bool none = m_new == -INFINITY;
+                alpha[h] = none ? 1.f : ex2_approx(m_run[h] - m_new);          // 0 on the first tile (m_run = -inf)
+                neg_m[h] = none ? 0.f : -m_new;
+                m_run[h] = m_new;
+            }
+            uint32_t a[BK / 16][4];
+            float lsum[2] = { 0.f, 0.f };
+#pragma unroll
+            for (int c = 0; c < BK / 8; c++) {
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const float p0 = ex2_approx(s[4 * c + 2 * h] + neg_m[h]);
+                    const float p1 = ex2_approx(s[4 * c + 2 * h + 1] + neg_m[h]);
+                    lsum[h] += p0 + p1;
+                    a[c >> 1][(c & 1) * 2 + h] = pack_half2(p0, p1);
+                }
+            }
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                l_run[h] = l_run[h] * alpha[h] + lsum[h];
+#pragma unroll
+                for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+                    for (int c = 0; c < 8; c++) { o[ch][4 * c + 2 * h] *= alpha[h]; o[ch][4 * c + 2 * h + 1] *= alpha[h]; }
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < BK / 16; kk++)
+#pragma unroll
+                for (int ch = 0; ch < NCH; ch++)
+                    wgmma_m64n64k16_f16_rs(o[ch], a[kk], vdesc0 + (uint64_t)((ks * C::KV_BYTES + ch * C::KV_CHUNK + kk * 2048) >> 4), 1u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            mbar_arrive(&kv_empty[ks]);
+        }
+        // epilogue: O / l -> fp16 -> out[hk][R][col]
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            float l = l_run[h];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = 1.f / l;
+            const int R = r0 + wg * (BQ / 2) + r + 8 * h;
+            if (R >= p.rows) continue;
+            __half* orow = p.out + ((long long)hk * p.rows + R) * p.d;
+#pragma unroll
+            for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+                for (int c = 0; c < 8; c++) {
+                    const int col = 64 * ch + 8 * c + cq;
+                    if (col < p.d)     // d % 8 == 0: the pair is inside
+                        *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
+                }
+        }
+    }
+}
+
+// [heads, rows, d] contiguous viewed as (d, rows, heads); box (64, box_rows, 1)
+bool sdpa_map(CUtensorMap* map, const void* base, int d, int64_t rows, int64_t heads, uint32_t box_rows)
+{
+    auto enc = fa_encode();
+    if (!enc) return false;
+    cuuint64_t dims[3] = { (cuuint64_t)d, (cuuint64_t)rows, (cuuint64_t)heads };
+    cuuint64_t strides[2] = { (cuuint64_t)d * 2, (cuuint64_t)rows * d * 2 };
+    cuuint32_t box[3] = { 64, box_rows, 1 };
+    cuuint32_t estr[3] = { 1, 1, 1 };
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+template <int NCH, int BK>
+int sdpa_launch(const void* q, const void* k, const void* v, const SdpaParams& p, int64_t Hkv, cudaStream_t st)
+{
+    using C = SdpaCfg<NCH, BK>;
+    CUtensorMap mq, mk, mv;
+    if (!sdpa_map(&mq, q, p.d, p.rows, Hkv, BQ) || !sdpa_map(&mk, k, p.d, p.Tk, Hkv, BK) || !sdpa_map(&mv, v, p.d, p.Tk, Hkv, BK))
+        return (int)cudaErrorInvalidValue;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(sdpa_flash_kernel<NCH, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
+        if (e != cudaSuccess) return (int)e;
+        attr = true;
+    }
+    SdpaParams pp = p;
+    pp.kv_tiles = (p.Tk + BK - 1) / BK;
+    dim3 grid((unsigned)((p.rows + BQ - 1) / BQ), (unsigned)Hkv);
+    osb_launch((sdpa_flash_kernel<NCH, BK>), grid, FA_THREADS, (size_t)C::SMEM, st, mq, mk, mv, pp);
+    return launched(1);
+}
+
 }  // namespace
 
 extern "C" int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
@@ -271,4 +536,25 @@ extern "C" int osb_flash_attention(const void* q, int64_t ldq, const void* k, in
     dim3 grid((unsigned)p.q_tiles, (unsigned)heads);
     osb_launch((flash_attention_kernel), grid, FA_THREADS, (size_t)FA_SMEM, st, mq, mk, mv, p);
     return launched(1);
+}
+
+extern "C" int osb_sdpa_flash_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, int dtype)
+{
+    return dtype == OSB_F16 && d == dv && d >= 8 && d <= 128 && d % 8 == 0 && Hkv >= 1 && Hkv <= 65535 && Hq >= Hkv && Hq % Hkv == 0 &&
+           Tq >= 1 && Tk >= 1 && (Hq / Hkv) * Tq <= (int64_t)INT32_MAX - BQ && Tk <= (int64_t)INT32_MAX - BKV && fa_encode() != nullptr;
+}
+
+// q [Hq,Tq,d], k / v [Hkv,Tk,d], mask [Tq,Tk] (additive, may be null), out [Hq,Tq,d]; fp16, contiguous.
+extern "C" int osb_sdpa_flash(const void* q, const void* k, const void* v, const void* mask, void* out,
+                              int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, float scale, void* stream)
+{
+    if (Hq * Tq * d == 0) return 0;
+    if (!osb_sdpa_flash_ok(Hq, Hkv, Tq, Tk, d, d, OSB_F16)) return (int)cudaErrorInvalidValue;
+    if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) != 0 || ((uintptr_t)mask & 3) != 0) return (int)cudaErrorInvalidValue;
+    SdpaParams p{};
+    p.rows = (int)((Hq / Hkv) * Tq); p.Tq = (int)Tq; p.Tk = (int)Tk; p.d = (int)d;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    p.mask = (const __half*)mask; p.out = (__half*)out;
+    cudaStream_t st = (cudaStream_t)stream;
+    return d <= 64 ? sdpa_launch<1, 128>(q, k, v, p, Hkv, st) : sdpa_launch<2, 64>(q, k, v, p, Hkv, st);
 }

@@ -812,7 +812,16 @@ struct Engine::Impl {
         if (!feeds(cc, m2, 0) || m2.in[1].wtype != DType::none) return 0;                                         // Mul(rot, sin)
         if (!feeds(m1, ad, 0) || !feeds(m2, ad, 1)) return 0;
         auto n_of = [](const TensorRef& r) { int64_t n = 1; for (auto d : r.shape) n *= d; return n; };
-        if (n_of(m1.in[1]) != D || n_of(m2.in[1]) != D) return 0;               // one cos / sin row shared by every head
+        // cos / sin: one row shared by every head (decode), or one row per position of x [.., heads, T, D] (prefill), broadcast over the heads
+        const int64_t T = xs.size() >= 2 ? xs[xs.size() - 2] : 1;
+        auto table_ok = [&](const TensorRef& r) {
+            const int64_t n = n_of(r);
+            if (n == D) return true;
+            if (n != T * D || r.shape.size() < 2 || r.shape.back() != D || r.shape[r.shape.size() - 2] != T) return false;
+            for (size_t k = 0; k + 2 < r.shape.size(); k++) if (r.shape[k] != 1) return false;
+            return true;
+        };
+        if (!table_ok(m1.in[1]) || !table_ok(m2.in[1])) return 0;
         auto it = uses.find(x);
         if (it == uses.end() || it->second != 3) return 0;                       // x: two Slices and the Mul
         for (int k = 0; k < 7; k++) if (upcast_op(ops[i + k])) return 0;
@@ -1723,6 +1732,11 @@ void Engine::Impl::op_concat(size_t oi)
     std::vector<int64_t> os = xs[0].shape;
     os[axis] = 0;
     for (auto& t : xs) { for (size_t d = 0; d < rank; d++) if ((int64_t)d != axis && t.shape[d] != xs[0].shape[d]) fail(op, "invalid shape of input."); os[axis] += t.shape[axis]; }
+    if (xs.size() == 2 && !nhwc_path) {
+        // one empty source (the first turn's zero-length KV cache): the result is the other source
+        for (int e = 0; e < 2; e++)
+            if (xs[e].numel() == 0) { Tensor r = xs[1 - e]; r.shape = os; push(oi, 0, r); return; }
+    }
     Tensor y = make(ty, os, nhwc_path ? Layout::nhwc : Layout::plain);
     y.scale = xs[0].scale; y.zero_point = xs[0].zero_point;
     // physical view: [outer, axis_len * inner]
@@ -2465,6 +2479,13 @@ void Engine::Impl::fused_sdpa(const Step& s)
     Tensor q3 = q, k3 = k, v3 = v;
     q3.shape = { Hq, Tq, D }; k3.shape = { Hkv, Tk, D }; v3.shape = { Hkv, Tk, Dv };
     Tensor o3 = out; o3.shape = { Hq, Tq, Dv };
+    // prompt prefill (more query rows than the decode kernels take): one fused wgmma kernel for all the grouped heads
+    const bool aligned = ((((uintptr_t)q.data() | (uintptr_t)k.data() | (uintptr_t)v.data() | (uintptr_t)out.data()) & 15) == 0) && (((uintptr_t)m.data() & 3) == 0);
+    if (q.type == DType::f16 && Tq > 16 && D == Dv && E.flash_attention && E.gemm_impl != 1 && aligned && osb_sdpa_flash_ok(Hq, Hkv, Tq, Tk, D, Dv, K(q.type))) {
+        ck(osb_sdpa_flash(q.data(), k.data(), v.data(), m.data(), out.mdata(), Hq, Hkv, Tq, Tk, D, scale, st), "osb_sdpa_flash");
+        push(i + 5, 0, out);
+        return;
+    }
     attention_core(q3, k3, v3, scale, false, &m, Hq / Hkv, o3);
     push(i + 5, 0, out);
 }
@@ -2562,11 +2583,15 @@ void Engine::Impl::fused_rope(const Step& s)
         return a == nd - 1 && (*sp.i64)[0] == 1 && (*st_.i64)[0] == lo && e == hi;
     };
     Tensor cs = to_plain(in(i + 4, 1)), sn = to_plain(in(i + 5, 1));
-    if (!cut(i, 0, D / 2) || !cut(i + 1, D / 2, D) || (x.type != DType::f16 && x.type != DType::f32) || cs.numel() != D || sn.numel() != D) { exec_unfused(s); return; }
+    // one table row for every x row, or one per position (x [.., T, D], table [T, D] broadcast over the leading dims)
+    const int64_t T = nd >= 2 ? x.shape[nd - 2] : 1;
+    const int64_t table_rows = cs.numel() / std::max<int64_t>(D, 1);
+    const bool table_ok = (table_rows == 1 || table_rows == T) && cs.numel() == table_rows * D && sn.numel() == cs.numel();
+    if (!cut(i, 0, D / 2) || !cut(i + 1, D / 2, D) || (x.type != DType::f16 && x.type != DType::f32) || !table_ok) { exec_unfused(s); return; }
     if (cs.type != x.type) cs = convert(cs, x.type);
     if (sn.type != x.type) sn = convert(sn, x.type);
     Tensor y = make(x.type, x.shape);
-    ck(osb_rope(x.data(), cs.data(), sn.data(), y.mdata(), K(x.type), x.numel() / D, D, 1, st), "osb_rope");
+    ck(osb_rope(x.data(), cs.data(), sn.data(), y.mdata(), K(x.type), x.numel() / D, D, table_rows, st), "osb_rope");
     push(i + 6, 0, y);
 }
 

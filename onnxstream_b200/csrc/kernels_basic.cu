@@ -899,7 +899,8 @@ __global__ void rope_kernel(const T* __restrict__ x, const T* __restrict__ cs, c
     const int half = D >> 1;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t r = i / D; const int j = (int)(i % D);
-        const int64_t t = table_rows == 1 ? 0 : r;
+        // one table row for every x row (decode), or x [.., T, D] cycling through T rows (prefill); no 64-bit division on the decode path
+        const int64_t t = table_rows == 1 ? 0 : (table_rows == rows ? r : r % table_rows);
         const float xv = to_float(x[i]);
         const float rot = j < half ? -to_float(x[i + half]) : to_float(x[i - half]);
         // the reference rounds each product and the sum to the storage type (three separate ops): keep those roundings
@@ -1532,7 +1533,7 @@ int osb_rms_norm(const void* x, int xd, const void* w, int wd, void* y, int yd, 
 int osb_rope(const void* x, const void* cs, const void* sn, void* y, int dtype, int64_t rows, int64_t D, int64_t table_rows, void* stream)
 {
     if (rows * D == 0) return 0;
-    if (D % 2 || (table_rows != 1 && table_rows != rows)) return (int)cudaErrorInvalidValue;
+    if (D % 2 || table_rows < 1 || rows % table_rows) return (int)cudaErrorInvalidValue;
     cudaStream_t st = (cudaStream_t)stream;
     if (dtype == OSB_F16) osb_launch((rope_kernel<__half>), grid_for((size_t)(rows * D), 256), 256, 0, st, (const __half*)x, (const __half*)cs, (const __half*)sn, (__half*)y, rows, (int)D, table_rows);
     else if (dtype == OSB_F32) osb_launch((rope_kernel<float>), grid_for((size_t)(rows * D), 256), 256, 0, st, (const float*)x, (const float*)cs, (const float*)sn, (float*)y, rows, (int)D, table_rows);
