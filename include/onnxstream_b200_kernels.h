@@ -192,7 +192,7 @@ int osb_attention(const void* q, const void* k, const void* v, const void* mask,
                   int64_t heads, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, float scale, int k_transposed,
                   int64_t kv_group, int dtype, void* stream);
 
-/* Fused flash-style multi-head attention on wgmma (fp16, d <= 64): q [T, heads*d] / k, v [Tk, heads*d] are read in place
+/* Fused flash-style multi-head attention on wgmma (fp16, d <= 160, d % 8 == 0): q [T, heads*d] / k, v [Tk, heads*d] are read in place
  * from the projection buffers (row strides ld*), out [T, heads*d] is written in the merged layout; the score tile lives in registers.
  * Covers the MatMul/Mul/Softmax/MatMul pattern plus the head split / merge around it (src/onnxstream.cpp:3576-3633, 6696-6929). */
 int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype);

@@ -4,15 +4,18 @@
 // src/onnxstream.cpp:6798-6799).
 //
 // One CTA per (head, 128-query tile), 384 threads:
-//   warpgroup 0      TMA producer (one warp): Q tile once, then a (K tile, V tile) pair per 128 keys into a KV_STAGES-deep ring
-//   warpgroups 1, 2  64 query rows each: S = Q K_j^T (wgmma m64n128k16 from shared memory, fp32 in registers), online softmax in
-//                    registers (fp32, exp2 with the scale folded in), P rounded to fp16 in registers is the A operand of O += P V_j
-//                    (wgmma m64n64k16, V from shared memory), finally O / sum -> fp16 -> global
+//   warpgroup 0      TMA producer (one warp, 40 registers): Q tile once, then a (K tile, V tile) pair per BK keys into a ring
+//   warpgroups 1, 2  64 query rows each (232 registers): S = Q K_j^T (wgmma from shared memory, fp32 in registers), online softmax
+//                    in registers (fp32, exp2 with the scale folded in), P rounded to fp16 in registers is the A operand of
+//                    O += P V_j (wgmma m64n64k16 per 64 output columns, V from shared memory), finally O / sum -> fp16 -> global
+// The consumer loop is software-pipelined: S_{j+1} = Q K_{j+1}^T and O += P_j V_j are issued together, and the softmax of S_{j+1} runs
+// while O += P_j V_j is in flight.  The two warpgroups take turns to issue their MMAs (two named barriers), so one warpgroup's
+// softmax overlaps the other's MMAs.
 // Q, K, V are read in place from the [T, heads*d] projection buffers through strided tensor maps and O is written in the
-// merged [T, heads*d] layout, so the exported graph's head split / merge costs nothing.  d <= 64, d % 8 == 0.
+// merged [T, heads*d] layout, so the exported graph's head split / merge costs nothing.  d <= 160, d % 8 == 0.
 //
-// sdpa_flash_kernel (below): the same structure for ScaledDotProductAttention with grouped KV heads and an additive mask -- llm.cpp's
-// prompt prefill -- for d <= 128.
+// sdpa_flash_kernel (below): the unpipelined structure for ScaledDotProductAttention with grouped KV heads and an additive mask --
+// llm.cpp's prompt prefill -- for d <= 128.
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -27,19 +30,29 @@ namespace {
 using namespace tcptx;
 
 constexpr int BQ = 128;                 // queries per CTA
-constexpr int BKV = 128;                // keys per tile
-constexpr int BD = 64;                  // head dim padded to one 128-byte swizzle row
+constexpr int BKV = 128;                // largest key tile
 constexpr int KV_STAGES = 4;            // K/V ring: the producer runs up to three tiles ahead of the slower warpgroup
-constexpr int Q_BYTES = BQ * BD * 2;    // 16 KiB
-constexpr int K_BYTES = BKV * BD * 2;   // 16 KiB
-constexpr int V_BYTES = BKV * BD * 2;   // 16 KiB (128 key rows x 64 columns)
-constexpr int FA_SMEM = Q_BYTES + KV_STAGES * (K_BYTES + V_BYTES) + 1024 + 256;
 constexpr int FA_THREADS = 384;
 constexpr int FA_CONSUMERS = 256;
+constexpr int FA_PRODUCER_REGS = 40, FA_CONSUMER_REGS = 232;     // 128 * 40 + 256 * 232 = 168 * 384: the whole register file
+
+// Tiling of flash_attention_kernel by head dim.  NCH = 64-column chunks of the head dim (one 128-byte swizzle row each; columns past d are
+// zero-filled by TMA), BK = keys per tile, QKS = k-steps of 16 in Q K^T (ceil(d / 16) rounded to an instantiation).  Registers per
+// consumer thread: O 32 * NCH, S BK / 2, P BK / 4 -- d <= 64: 128-key tiles (32 + 64 + 32), d <= 128: 64-key tiles (64 + 32 + 16),
+// d <= 160: 32-key tiles (96 + 16 + 8; with 64-key tiles ptxas spills and serialises the wgmmas).
+template <int NCH, int BK, int QKS>
+struct FaCfg {
+    static_assert(QKS <= 4 * NCH && (BK == 32 || BK == 64 || BK == 128), "tile");
+    static constexpr int Q_CHUNK = BQ * 128;            // 128 rows x 64 fp16 columns
+    static constexpr int KV_CHUNK = BK * 128;
+    static constexpr int Q_BYTES = NCH * Q_CHUNK;
+    static constexpr int KV_BYTES = NCH * KV_CHUNK;     // one K (or V) tile
+    static constexpr int SMEM = Q_BYTES + KV_STAGES * 2 * KV_BYTES + 1024 + 256;
+};
 
 struct FaParams {
-    int T, Tk, d, heads;
-    int q_tiles, kv_tiles;
+    int T, Tk, d;
+    int kv_tiles;
     float scale_log2;        // scale * log2(e)
     float tau;               // lazy-rescaling threshold in log2 units (0 = exact running maximum)
     __half* out;             // [T, ldo] merged layout, head h at column h*d
@@ -61,24 +74,129 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi)
     return *reinterpret_cast<uint32_t*>(&h2);
 }
 
+template <int BK>
+__device__ __forceinline__ void qk_mma(float (&s)[BK / 2], uint64_t da, uint64_t db, uint32_t scale_d = 1u)
+{
+    if constexpr (BK == 128) wgmma_m64n128k16_f16<0>(s, da, db, scale_d);
+    else if constexpr (BK == 64) wgmma_m64n64k16_f16<0>(s, da, db, scale_d);
+    else wgmma_m64n32k16_f16<0>(s, da, db, scale_d);
+}
+
+// S = Q K^T for one key tile (kdesc: the tile's first chunk), issued as one wgmma group.  Q / K K-major: 32 B per 16-element k-step inside
+// a 64-column chunk; the first k-step overwrites S.
+template <int NCH, int BK, int QKS>
+__device__ __forceinline__ void fa_issue_qk(float (&s)[BK / 2], uint64_t qdesc, uint64_t kdesc)
+{
+    using C = FaCfg<NCH, BK, QKS>;
+    fence_regs(s);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < QKS; k++)
+        qk_mma<BK>(s, qdesc + (uint64_t)(((k >> 2) * C::Q_CHUNK >> 4) + (k & 3) * 2), kdesc + (uint64_t)(((k >> 2) * C::KV_CHUNK >> 4) + (k & 3) * 2), k > 0);
+    wgmma_commit();
+}
+
+// O += P V for one key tile (vdesc: the tile's first chunk), one wgmma group.  V MN-major: 16 keys = 2048 B per k-step.
+template <int NCH, int BK, int QKS>
+__device__ __forceinline__ void fa_issue_pv(float (&o)[NCH][32], uint32_t (&a)[BK / 16][4], uint64_t vdesc)
+{
+    using C = FaCfg<NCH, BK, QKS>;
+#pragma unroll
+    for (int ch = 0; ch < NCH; ch++) fence_regs(o[ch]);
+    fence_regs(a);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; kk++)
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++)
+            wgmma_m64n64k16_f16_rs(o[ch], a[kk], vdesc + (uint64_t)((ch * C::KV_CHUNK + kk * 2048) >> 4), 1u);
+    wgmma_commit();
+}
+
+// Online softmax of one score tile in place: padding keys (the last tile only; K rows zero-filled by TMA) get -inf, the running maximum
+// and this thread's partial row sums advance, s becomes p = 2^(s*scale*log2e - m_new) in fp32 and alpha the factor that rescales O.
+// Accumulator fragments (tc_ptx.cuh): this thread holds rows r and r + 8 of the warpgroup's 64 (h = 0, 1) and, per 8-column block c,
+// the columns 8c + cq, 8c + cq + 1.  The four lanes of a row share its maximum by two shuffles.
+template <int BK>
+__device__ __forceinline__ void fa_softmax(float (&s)[BK / 2], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2], int key0, int cq, const FaParams& p)
+{
+    if (key0 + BK > p.Tk) {
+#pragma unroll
+        for (int c = 0; c < BK / 8; c++)
+#pragma unroll
+            for (int e = 0; e < 2; e++)
+                if (key0 + 8 * c + cq + e >= p.Tk) { s[4 * c + e] = -INFINITY; s[4 * c + 2 + e] = -INFINITY; }
+    }
+    float neg_m[2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float mt = -INFINITY;
+#pragma unroll
+        for (int c = 0; c < BK / 8; c++) mt = fmaxf(mt, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
+        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+        // Lazy rescaling: the stale maximum is kept while the new one exceeds it by at most tau (log2 units) -- P <= 2^tau stays well
+        // inside fp16, O and l accumulate in fp32.  tau = 0 is the exact running maximum (the default; OSB_FLASH_TAU sets it).
+        const float m_cand = fmaxf(m_run[h], mt * p.scale_log2);     // scale_log2 > 0
+        const float m_new = (m_cand - m_run[h] > p.tau) ? m_cand : m_run[h];
+        alpha[h] = ex2_approx(m_run[h] - m_new);                     // 0 on the first tile (m_run = -inf)
+        neg_m[h] = -m_new;
+        m_run[h] = m_new;
+    }
+    // one FFMA + one MUFU.EX2 per score
+    float lsum[2] = { 0.f, 0.f };
+#pragma unroll
+    for (int c = 0; c < BK / 8; c++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const float pe = ex2_approx(fmaf(s[4 * c + 2 * h + e], p.scale_log2, neg_m[h]));
+                s[4 * c + 2 * h + e] = pe;
+                lsum[h] += pe;
+            }
+#pragma unroll
+    for (int h = 0; h < 2; h++) l_run[h] = l_run[h] * alpha[h] + lsum[h];    // this thread's partial row sum (the quad shares alpha)
+}
+
+// O *= alpha, then P (fp32 in s) rounded to fp16 in the A-fragment order of the PV MMA (k-step kk covers keys 16kk..16kk+15 = blocks
+// 2kk, 2kk+1: {block 2kk row r, row r+8, block 2kk+1 row r, row r+8})
+template <int NCH, int BK>
+__device__ __forceinline__ void fa_rescale_pack(float (&o)[NCH][32], uint32_t (&a)[BK / 16][4], const float (&s)[BK / 2], const float (&alpha)[2])
+{
+#pragma unroll
+    for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+        for (int c = 0; c < 8; c++)
+#pragma unroll
+            for (int h = 0; h < 2; h++) { o[ch][4 * c + 2 * h] *= alpha[h]; o[ch][4 * c + 2 * h + 1] *= alpha[h]; }
+#pragma unroll
+    for (int c = 0; c < BK / 8; c++)
+#pragma unroll
+        for (int h = 0; h < 2; h++) a[c >> 1][(c & 1) * 2 + h] = pack_half2(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]);
+}
+
+template <int NCH, int BK, int QKS>
 __global__ void __launch_bounds__(FA_THREADS, 1)
 flash_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
                        const FaParams p)
 {
+    using C = FaCfg<NCH, BK, QKS>;
+    constexpr int S = KV_STAGES;
     osb_pdl_trigger_entry();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* sQ = smem;
-    uint8_t* sK = sQ + Q_BYTES;
-    uint8_t* sV = sK + KV_STAGES * K_BYTES;
-    uint64_t* bars = (uint64_t*)(sV + KV_STAGES * V_BYTES);
+    uint8_t* sK = sQ + C::Q_BYTES;
+    uint8_t* sV = sK + S * C::KV_BYTES;
+    uint64_t* bars = (uint64_t*)(sV + S * C::KV_BYTES);
     uint64_t* q_full = bars;                           // [1]
-    uint64_t* kv_full = bars + 1;                      // [KV_STAGES]
-    uint64_t* kv_empty = kv_full + KV_STAGES;          // [KV_STAGES]
+    uint64_t* kv_full = bars + 1;                      // [S]
+    uint64_t* kv_empty = kv_full + S;                  // [S]: one arrival per consumer warp
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int qt = blockIdx.x, head = blockIdx.y;
-    const int q0 = qt * BQ;
+    const int head = blockIdx.y;
+    const int q0 = blockIdx.x * BQ;
 
     if (warp == 0 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
@@ -87,7 +205,7 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_c
     }
     if (warp == 1 && lane == 0) {
         mbar_init(q_full, 1);
-        for (int i = 0; i < KV_STAGES; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], FA_CONSUMERS); }
+        for (int i = 0; i < S; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], FA_CONSUMERS / 32); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -95,104 +213,88 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_c
 
     const int n_kv = p.kv_tiles;
 
-    if (warp == 0) {
-        if (elect_one()) {
-            mbar_expect_tx(q_full, Q_BYTES);
-            tma_load_3d(sQ, &map_q, q_full, 0, head, q0);
-        }
-        __syncwarp();
-        for (int j = 0; j < n_kv; j++) {
-            const int st = j % KV_STAGES;
-            mbar_wait(&kv_empty[st], ((j / KV_STAGES) & 1) ^ 1);
+    if (warp < 4) {
+        setmaxnreg_dec<FA_PRODUCER_REGS>();
+        if (warp == 0) {
             if (elect_one()) {
-                mbar_expect_tx(&kv_full[st], K_BYTES + V_BYTES);
-                tma_load_3d(sK + st * K_BYTES, &map_k, &kv_full[st], 0, head, j * BKV);
-                tma_load_3d(sV + st * V_BYTES, &map_v, &kv_full[st], 0, head, j * BKV);
-                tma_load_3d(sV + st * V_BYTES + V_BYTES / 2, &map_v, &kv_full[st], 0, head, j * BKV + 64);
+                mbar_expect_tx(q_full, C::Q_BYTES);
+#pragma unroll
+                for (int c = 0; c < NCH; c++) tma_load_3d(sQ + c * C::Q_CHUNK, &map_q, q_full, 64 * c, head, q0);
             }
             __syncwarp();
+            for (int j = 0; j < n_kv; j++) {
+                const int st = j % S;
+                mbar_wait(&kv_empty[st], ((j / S) & 1) ^ 1);
+                if (elect_one()) {
+                    mbar_expect_tx(&kv_full[st], 2 * C::KV_BYTES);
+#pragma unroll
+                    for (int c = 0; c < NCH; c++) {
+                        tma_load_3d(sK + st * C::KV_BYTES + c * C::KV_CHUNK, &map_k, &kv_full[st], 64 * c, head, j * BK);
+                        tma_load_3d(sV + st * C::KV_BYTES + c * C::KV_CHUNK, &map_v, &kv_full[st], 64 * c, head, j * BK);
+                    }
+                }
+                __syncwarp();
+            }
         }
-    } else if (warp >= 4) {
+    } else {
         // ===================== warpgroups 1, 2: 64 query rows each =====================
-        // Accumulator fragments (tc_ptx.cuh): this thread holds rows r and r + 8 of the warpgroup's 64 (h = 0, 1) and, per 8-column
-        // block c, the columns 8c + cq, 8c + cq + 1 -- of the 128 keys in s[], of the 64 output columns in o[].  The four lanes of a row
-        // share its maximum and sum by two shuffles.
+        setmaxnreg_inc<FA_CONSUMER_REGS>();
         const int wg = (warp >> 2) - 1;
         const int r = (warp & 3) * 16 + (lane >> 2);
         const int cq = 2 * (lane & 3);
-        // descriptors (start address in 16-byte units moves): Q / K K-major, 8-row groups 1024 B apart, 32 B per 16-element K step;
-        // V MN-major (key rows of 64 columns = one atom), 8-key groups 1024 B apart, 16 keys = 2048 B per K step
+        // Turn-taking: warpgroup w waits on named barrier 1 + w (its own 128 threads + the other's 128 arrivals) before it issues MMAs
+        // and arrives on the other's barrier after.  Warpgroup 0 pre-arrives on its own barrier to take the first turn, so warpgroup 1's
+        // last arrival would have no matching wait and is left out.
+        const uint32_t my_bar = 1 + wg, other_bar = 2 - wg;
+        if (wg == 0) named_bar_arrive(my_bar, FA_CONSUMERS);
+        // descriptors (start address in 16-byte units moves): Q / K K-major, 8-row groups 1024 B apart; V MN-major, 8-key groups 1024 B apart
         const uint64_t qdesc = make_smem_desc(smem_u32(sQ) + wg * (BQ / 2) * 128, 16, 1024);
         const uint64_t kdesc0 = make_smem_desc(smem_u32(sK), 16, 1024);
-        const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), V_BYTES, 1024);
-        float o[32];
+        const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), C::KV_CHUNK, 1024);
+        float o[NCH][32];
 #pragma unroll
-        for (int i = 0; i < 32; i++) o[i] = 0.f;
-        float m_run[2] = { -INFINITY, -INFINITY }, l_run[2] = { 0.f, 0.f };
+        for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+            for (int i = 0; i < 32; i++) o[ch][i] = 0.f;
+        float s[BK / 2];
+        uint32_t a[BK / 16][4];
+        float m_run[2] = { -INFINITY, -INFINITY }, l_run[2] = { 0.f, 0.f }, alpha[2];
         mbar_wait(q_full, 0);
-        for (int j = 0; j < n_kv; j++) {
-            const int ks = j % KV_STAGES;
-            mbar_wait(&kv_full[ks], (j / KV_STAGES) & 1);
-            float s[64];
-#pragma unroll
-            for (int i = 0; i < 64; i++) s[i] = 0.f;
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < BD / 16; k++) wgmma_m64n128k16_f16<0>(s, qdesc + (uint64_t)(k * 2), kdesc0 + (uint64_t)(ks * (K_BYTES >> 4) + k * 2), 1u);
-            wgmma_commit();
+
+        // tile 0: S_0, its softmax, P_0
+        mbar_wait(&kv_full[0], 0);
+        named_bar_sync(my_bar, FA_CONSUMERS);
+        fa_issue_qk<NCH, BK, QKS>(s, qdesc, kdesc0);
+        named_bar_arrive(other_bar, FA_CONSUMERS);
+        wgmma_wait<0>();
+        fence_regs(s);
+        fa_softmax<BK>(s, m_run, l_run, alpha, 0, cq, p);
+        fa_rescale_pack<NCH, BK>(o, a, s, alpha);
+        // tile j: S_j and O += P_{j-1} V_{j-1} in flight together; the softmax of S_j waits for S_j only
+        for (int j = 1; j < n_kv; j++) {
+            const int st = j % S, prev = (j - 1) % S;
+            mbar_wait(&kv_full[st], (j / S) & 1);
+            named_bar_sync(my_bar, FA_CONSUMERS);
+            fa_issue_qk<NCH, BK, QKS>(s, qdesc, kdesc0 + (uint64_t)(st * C::KV_BYTES >> 4));
+            fa_issue_pv<NCH, BK, QKS>(o, a, vdesc0 + (uint64_t)(prev * C::KV_BYTES >> 4));
+            named_bar_arrive(other_bar, FA_CONSUMERS);
+            wgmma_wait<1>();
+            fence_regs(s);
+            fa_softmax<BK>(s, m_run, l_run, alpha, j * BK, cq, p);
             wgmma_wait<0>();
-            // only the last tile has padding keys (K rows zero-filled by TMA): they get probability 0
-            if (j * BKV + BKV > p.Tk) {
 #pragma unroll
-                for (int c = 0; c < BKV / 8; c++)
-#pragma unroll
-                    for (int e = 0; e < 2; e++)
-                        if (j * BKV + 8 * c + cq + e >= p.Tk) { s[4 * c + e] = -INFINITY; s[4 * c + 2 + e] = -INFINITY; }
-            }
-            float alpha[2], neg_m[2];
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                float mt = -INFINITY;
-#pragma unroll
-                for (int c = 0; c < BKV / 8; c++) mt = fmaxf(mt, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
-                mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
-                mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
-                // Lazy rescaling: the stale maximum is kept while the new one exceeds it by at most tau (log2 units) -- P <= 2^tau stays well
-                // inside fp16, O and l accumulate in fp32.  tau = 0 is the exact running maximum (the default; OSB_FLASH_TAU sets it).
-                const float m_cand = fmaxf(m_run[h], mt * p.scale_log2);     // scale_log2 > 0
-                const float m_new = (m_cand - m_run[h] > p.tau) ? m_cand : m_run[h];
-                alpha[h] = ex2_approx(m_run[h] - m_new);                     // 0 on the first tile (m_run = -inf)
-                neg_m[h] = -m_new;
-                m_run[h] = m_new;
-            }
-            // p = 2^(s*scale*log2e - m_new): one FFMA + one MUFU.EX2 per score, packed to fp16 in the A-fragment order of the PV MMA
-            // (k-step kk covers keys 16kk..16kk+15 = blocks 2kk, 2kk+1: {block 2kk row r, row r+8, block 2kk+1 row r, row r+8})
-            uint32_t a[BKV / 16][4];
-            float lsum[2] = { 0.f, 0.f };
-#pragma unroll
-            for (int c = 0; c < BKV / 8; c++) {
-#pragma unroll
-                for (int h = 0; h < 2; h++) {
-                    const float p0 = ex2_approx(fmaf(s[4 * c + 2 * h], p.scale_log2, neg_m[h]));
-                    const float p1 = ex2_approx(fmaf(s[4 * c + 2 * h + 1], p.scale_log2, neg_m[h]));
-                    lsum[h] += p0 + p1;
-                    a[c >> 1][(c & 1) * 2 + h] = pack_half2(p0, p1);
-                }
-            }
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                l_run[h] = l_run[h] * alpha[h] + lsum[h];    // this thread's partial row sum (the quad shares alpha)
-#pragma unroll
-                for (int c = 0; c < BD / 8; c++) { o[4 * c + 2 * h] *= alpha[h]; o[4 * c + 2 * h + 1] *= alpha[h]; }
-            }
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < BKV / 16; kk++)
-                wgmma_m64n64k16_f16_rs(o, a[kk], vdesc0 + (uint64_t)(ks * (V_BYTES >> 4) + kk * (2048 >> 4)), 1u);
-            wgmma_commit();
-            wgmma_wait<0>();
-            mbar_arrive(&kv_empty[ks]);
+            for (int ch = 0; ch < NCH; ch++) fence_regs(o[ch]);
+            fence_regs(a);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&kv_empty[prev]);
+            fa_rescale_pack<NCH, BK>(o, a, s, alpha);
         }
+        named_bar_sync(my_bar, FA_CONSUMERS);
+        fa_issue_pv<NCH, BK, QKS>(o, a, vdesc0 + (uint64_t)((n_kv - 1) % S * C::KV_BYTES >> 4));
+        if (wg == 0) named_bar_arrive(other_bar, FA_CONSUMERS);
+        wgmma_wait<0>();
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++) fence_regs(o[ch]);
         // epilogue: O / l -> fp16 -> out[q, head*d + c]
 #pragma unroll
         for (int h = 0; h < 2; h++) {
@@ -204,11 +306,13 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_c
             if (qrow >= p.T) continue;
             __half* orow = p.out + (long long)qrow * p.ldo + (long long)head * p.d;
 #pragma unroll
-            for (int c = 0; c < BD / 8; c++) {
-                const int col = 8 * c + cq;
-                if (col < p.d)     // d % 8 == 0: the pair is inside
-                    *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[4 * c + 2 * h] * inv, o[4 * c + 2 * h + 1] * inv);
-            }
+            for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+                for (int c = 0; c < 8; c++) {
+                    const int col = 64 * ch + 8 * c + cq;
+                    if (col < p.d)     // d % 8 == 0: the pair is inside
+                        *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
+                }
         }
     }
 }
@@ -276,13 +380,6 @@ __device__ __forceinline__ uint32_t ld_mask_pair(const __half* row, int col, int
         return (uint32_t)__ldg(m) | ((uint32_t)__ldg(m + 1) << 16);
     }
     return col < Tk ? (uint32_t)__ldg(m) : 0u;
-}
-
-template <int BK>
-__device__ __forceinline__ void qk_mma(float (&s)[BK / 2], uint64_t da, uint64_t db)
-{
-    if constexpr (BK == 128) wgmma_m64n128k16_f16<0>(s, da, db, 1u);
-    else wgmma_m64n64k16_f16<0>(s, da, db, 1u);
 }
 
 template <int NCH, int BK>
@@ -501,11 +598,32 @@ int sdpa_launch(const void* q, const void* k, const void* v, const SdpaParams& p
     return launched(1);
 }
 
+// K and V tensor maps take BK-row boxes, Q 128-row boxes; each box is 64 columns wide (one chunk)
+template <int NCH, int BK, int QKS>
+int fa_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, FaParams p, int64_t heads, cudaStream_t st)
+{
+    using C = FaCfg<NCH, BK, QKS>;
+    CUtensorMap mq, mk, mv;
+    if (!head_map(&mq, q, p.d, (int)heads, p.T, ldq, BQ) || !head_map(&mk, k, p.d, (int)heads, p.Tk, ldk, BK) ||
+        !head_map(&mv, v, p.d, (int)heads, p.Tk, ldv, BK))
+        return (int)cudaErrorInvalidValue;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(flash_attention_kernel<NCH, BK, QKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
+        if (e != cudaSuccess) return (int)e;
+        attr = true;
+    }
+    p.kv_tiles = (p.Tk + BK - 1) / BK;
+    dim3 grid((unsigned)((p.T + BQ - 1) / BQ), (unsigned)heads);
+    osb_launch((flash_attention_kernel<NCH, BK, QKS>), grid, FA_THREADS, (size_t)C::SMEM, st, mq, mk, mv, p);
+    return launched(1);
+}
+
 }  // namespace
 
 extern "C" int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
 {
-    return dtype == OSB_F16 && d >= 8 && d <= 64 && d % 8 == 0 && T >= 64 && Tk >= 1 && fa_encode() != nullptr;
+    return dtype == OSB_F16 && d >= 8 && d <= 160 && d % 8 == 0 && T >= 64 && Tk >= 1 && fa_encode() != nullptr;
 }
 
 // q [T, heads*d] (row stride ldq), k / v [Tk, heads*d] (row strides ldk / ldv), out [T, heads*d] (row stride ldo); fp16.
@@ -513,29 +631,20 @@ extern "C" int osb_flash_attention(const void* q, int64_t ldq, const void* k, in
                                    int64_t heads, int64_t T, int64_t Tk, int64_t d, float scale, void* stream)
 {
     if (heads * T == 0) return 0;
-    if (d > 64 || d % 8 || (ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 8)) return (int)cudaErrorInvalidValue;
+    if (d < 8 || d > 160 || d % 8 || Tk < 1 || (ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 8)) return (int)cudaErrorInvalidValue;
     if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) != 0) return (int)cudaErrorInvalidValue;
-    cudaStream_t st = (cudaStream_t)stream;
-    CUtensorMap mq, mk, mv;
-    if (!head_map(&mq, q, (int)d, (int)heads, T, ldq, BQ)) return (int)cudaErrorInvalidValue;
-    if (!head_map(&mk, k, (int)d, (int)heads, Tk, ldk, BKV)) return (int)cudaErrorInvalidValue;
-    if (!head_map(&mv, v, (int)d, (int)heads, Tk, ldv, 64)) return (int)cudaErrorInvalidValue;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(flash_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM);
-        if (e != cudaSuccess) return (int)e;
-        attr = true;
-    }
     FaParams p{};
-    p.T = (int)T; p.Tk = (int)Tk; p.d = (int)d; p.heads = (int)heads;
-    p.q_tiles = (int)((T + BQ - 1) / BQ); p.kv_tiles = (int)((Tk + BKV - 1) / BKV);
+    p.T = (int)T; p.Tk = (int)Tk; p.d = (int)d;
     p.scale_log2 = scale * 1.4426950408889634f;
     static const float tau_env = [] { const char* e = getenv("OSB_FLASH_TAU"); float v = e ? (float)atof(e) : 0.f; return v < 0.f ? 0.f : (v > 12.f ? 12.f : v); }();
     p.tau = tau_env;
     p.out = (__half*)out; p.ldo = ldo;
-    dim3 grid((unsigned)p.q_tiles, (unsigned)heads);
-    osb_launch((flash_attention_kernel), grid, FA_THREADS, (size_t)FA_SMEM, st, mq, mk, mv, p);
-    return launched(1);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (d <= 48) return fa_launch<1, 128, 3>(q, ldq, k, ldk, v, ldv, p, heads, st);
+    if (d <= 64) return fa_launch<1, 128, 4>(q, ldq, k, ldk, v, ldv, p, heads, st);
+    if (d <= 80) return fa_launch<2, 64, 5>(q, ldq, k, ldk, v, ldv, p, heads, st);
+    if (d <= 128) return fa_launch<2, 64, 8>(q, ldq, k, ldk, v, ldv, p, heads, st);
+    return fa_launch<3, 32, 10>(q, ldq, k, ldk, v, ldv, p, heads, st);
 }
 
 extern "C" int osb_sdpa_flash_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, int dtype)

@@ -199,7 +199,7 @@ public:
     bool fuse_nodes = true;          // GroupNorm/LayerNorm/GELU/SiLU/bias/residual fusions
     bool keep_nhwc = true;           // keep conv trunks channel-last instead of transposing around every Conv
     int gemm_impl = 0;               // 0 auto, 1 force CUDA-core kernels, 2 force the tensor-core kernel
-    bool flash_attention = true;     // fused wgmma attention: multi-head blocks with d <= 64 (else two GEMMs around a softmax), SDPA prefill with d <= 128
+    bool flash_attention = true;     // fused wgmma attention: multi-head blocks with d <= 160 (else two GEMMs around a softmax), SDPA prefill with d <= 128
     double ring_factor = 1.0;        // weight ring capacity = ring_factor * largest node footprint
     bool keep_inputs = false;        // graph inputs stay in HBM after a run; a later run that does not push a name again reuses the device copy
                                      // (a device-resident KV cache for fixed-shape decode steps: only the new token's ids cross PCIe)

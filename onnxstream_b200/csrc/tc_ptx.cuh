@@ -88,6 +88,32 @@ __device__ __forceinline__ bool elect_one()
     return pred != 0;
 }
 
+// named barrier over `count` threads (id 0 is __syncthreads): sync waits for the count, arrive adds this warp's threads and goes on
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+
+// per-thread register budget of the executing warpgroup (every warp of it executes the instruction)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// pins registers that an asynchronous wgmma reads or writes: the compiler may not move their other uses across this point
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N])
+{
+#pragma unroll
+    for (int i = 0; i < N; i++) asm volatile("" : "+f"(r[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[N][4])
+{
+#pragma unroll
+    for (int i = 0; i < N; i++)
+#pragma unroll
+        for (int e = 0; e < 4; e++) asm volatile("" : "+r"(r[i][e])::"memory");
+}
+
 // shared-memory matrix descriptor for wgmma (cute/arch/mma_sm90_desc.hpp GmmaDescriptor): 128B swizzle, start / LBO / SBO in 16-byte units.
 //   K-major: 8-row groups SBO bytes apart (LBO unused).  MN-major: 64-element MN atoms LBO bytes apart, 8-row K groups SBO bytes apart.
 // Every operand tile starts on a 1024-byte boundary, so the base-offset field stays 0; advancing K inside a swizzle row adds to the start address.
@@ -128,6 +154,16 @@ __device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t da,
         "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, %35;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
+}
+template <int TRANS_B>
+__device__ __forceinline__ void wgmma_m64n32k16_f16(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, %19;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
         : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
 }
 template <int TRANS_B>
