@@ -486,6 +486,18 @@ __global__ void inorm_apply_kernel(const T* __restrict__ x, T* __restrict__ y, c
 // GroupNorm (+SiLU) on [C, HW] (NCHW) or [HW, C] (NHWC)
 // ------------------------------------------------------------------------------------------------------------
 
+// osb_group_norm's statistics are taken around a per-group pivot p, the group's first element in memory (NHWC: its first channel at
+// pixel 0; NCHW: the start of its slab), which every CTA reads alike: stats = fp64 sums of the fp32 partials of x - p and (x - p)^2, and
+// the readers form mean = p + S/n, var = Q/n - (S/n)^2.  Plain sums of x and x^2 cancel in E[x^2] - mean^2 when the mean is large
+// against the spread (x = 1024 + N(0,1) in fp16: rstd up to 9 % off).  The stats stay fp64 sums of fp32 partials; only what is
+// summed moved, so the producers and the scratch layout are unchanged.
+__device__ __forceinline__ void gn_mean_var(const double* stats, int g, double inv_n, float p, double& mean, double& var)
+{
+    const double s = stats[2 * g] * inv_n;
+    mean = (double)p + s;
+    var = stats[2 * g + 1] * inv_n - s * s;
+}
+
 // NCHW: group g = contiguous slab of (C/G)*HW elements -> same as instance norm stats with C := G.
 // NHWC: each pixel row holds C channels; a CTA takes a strip of pixels, accumulates per-channel partials in registers
 // (thread t owns channels t, t+blockDim, ...), folds them to groups through shared memory, then atomically adds to stats.
@@ -499,9 +511,10 @@ __global__ void gn_stats_nhwc_kernel(const T* __restrict__ x, double* __restrict
     int64_t p0 = (int64_t)blockIdx.x * pix_per_cta, p1 = min(p0 + pix_per_cta, HW);
     int cpg = (int)(C / groups);
     for (int64_t c = threadIdx.x; c < C; c += blockDim.x) {
-        float s = 0.f, q = 0.f;
-        for (int64_t p = p0; p < p1; p++) { float v = to_float(x[p * C + c]); s += v; q += v * v; }
         int g = (int)(c / cpg);
+        const float pv = to_float(x[(int64_t)g * cpg]);
+        float s = 0.f, q = 0.f;
+        for (int64_t p = p0; p < p1; p++) { float v = to_float(x[p * C + c]) - pv; s += v; q += v * v; }
         atomicAdd(&sm[2 * g], s);
         atomicAdd(&sm[2 * g + 1], q);
     }
@@ -514,10 +527,11 @@ __global__ void gn_stats_nhwc_kernel(const T* __restrict__ x, double* __restrict
 // bins with shared-memory atomics, then one double atomic per bin and CTA.
 template <typename T, int VEC>
 __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __restrict__ stats, int C, int64_t HW, int groups, int64_t pix_per_cta,
-                                         const T* __restrict__ addv = nullptr, T* __restrict__ y = nullptr)
+                                         const T* __restrict__ addv = nullptr, T* __restrict__ y = nullptr, int pivot = 0)
 {
     // addv / y != null: y = x + addv[c] (the per-channel time-embedding add of a resnet) is written on the way and the statistics
-    // are those of y -- the producer side of a GroupNorm whose apply pass is gn_apply_pre_kernel
+    // are those of y -- the producer side of a GroupNorm whose apply pass is gn_apply_pre_kernel.  pivot != 0: sums of x - p around
+    // the group pivot (osb_group_norm's layout, see gn_mean_var); else plain sums, which gn_apply_pre_kernel reads
     osb_pdl_prologue();
     extern __shared__ float sm[];  // 2 * groups
     for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) sm[i] = 0.f;
@@ -526,10 +540,11 @@ __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __rest
     const int rows = blockDim.x / tpp;              // pixels in flight
     const int cv = threadIdx.x % tpp, pr = threadIdx.x / tpp;
     int64_t p0 = (int64_t)blockIdx.x * pix_per_cta, p1 = min(p0 + pix_per_cta, HW);
+    const int cpg = C / groups;
     if (pr < rows) {
-        float s[VEC], q[VEC], a[VEC];
+        float s[VEC], q[VEC], a[VEC], pv[VEC];
 #pragma unroll
-        for (int k = 0; k < VEC; k++) { s[k] = 0.f; q[k] = 0.f; a[k] = 0.f; }
+        for (int k = 0; k < VEC; k++) { s[k] = 0.f; q[k] = 0.f; a[k] = 0.f; pv[k] = pivot ? to_float(x[(cv * VEC + k) / cpg * cpg]) : 0.f; }
         if (addv) {
             Vec<T, VEC> av = load_vec<T, VEC>(addv + cv * VEC);
 #pragma unroll
@@ -550,7 +565,7 @@ __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __rest
                     store_vec<T, VEC>(y + p * C + cv * VEC, v[u]);
                 }
 #pragma unroll
-                for (int k = 0; k < VEC; k++) { float f = to_float(v[u].v[k]); s[k] += f; q[k] += f * f; }
+                for (int k = 0; k < VEC; k++) { float f = to_float(v[u].v[k]) - pv[k]; s[k] += f; q[k] += f * f; }
             }
         }
         // per-thread partials -> shared [rows][2][C] (no atomics: 256 threads hammering 2 * groups shared addresses serialise)
@@ -561,7 +576,6 @@ __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __rest
     __syncthreads();
     {
         // thread t < 2 * groups: group t / 2, statistic t % 2 -- sums its cpg channels over the pixel rows of the CTA
-        const int cpg = C / groups;
         const float* part = sm + 2 * groups;
         for (int t = threadIdx.x; t < 2 * groups; t += blockDim.x) {
             const int g = t >> 1, which = t & 1;
@@ -594,13 +608,13 @@ gn_fused_nhwc_kernel(const T* __restrict__ x, T* __restrict__ y, double* __restr
     const int cpg = C / groups;
     int64_t p0 = (int64_t)blockIdx.x * pix_per_cta, p1 = min(p0 + pix_per_cta, HW);
     if (pr < rows) {
-        float s[VEC], q[VEC];
+        float s[VEC], q[VEC], pv[VEC];
 #pragma unroll
-        for (int k = 0; k < VEC; k++) { s[k] = 0.f; q[k] = 0.f; }
+        for (int k = 0; k < VEC; k++) { s[k] = 0.f; q[k] = 0.f; pv[k] = to_float(x[(cv * VEC + k) / cpg * cpg]); }
         for (int64_t p = p0 + pr; p < p1; p += rows) {
             Vec<T, VEC> v = load_vec<T, VEC>(x + p * C + cv * VEC);
 #pragma unroll
-            for (int k = 0; k < VEC; k++) { float f = to_float(v.v[k]); s[k] += f; q[k] += f * f; }
+            for (int k = 0; k < VEC; k++) { float f = to_float(v.v[k]) - pv[k]; s[k] += f; q[k] += f * f; }
         }
         // combine the channels of this vector that fall into the same group in registers first: 2 (not 2 * VEC) shared atomics
         // per group touched -- the contended shared atomics were the longest phase of the kernel
@@ -635,8 +649,9 @@ gn_fused_nhwc_kernel(const T* __restrict__ x, T* __restrict__ y, double* __restr
     // ---- per-group mean / rstd into shared memory ----
     const double inv_n = 1.0 / (double)((int64_t)cpg * HW);
     for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-        double mean = __ldcg(&stats[2 * g]) * inv_n;
-        double var = __ldcg(&stats[2 * g + 1]) * inv_n - mean * mean;
+        const double s = __ldcg(&stats[2 * g]) * inv_n;
+        const double mean = (double)to_float(x[(int64_t)g * cpg]) + s;
+        const double var = __ldcg(&stats[2 * g + 1]) * inv_n - s * s;
         sm[2 * g] = (float)mean;
         sm[2 * g + 1] = rsqrtf(fmaxf((float)var, 0.f) + eps);
     }
@@ -680,8 +695,9 @@ __global__ void gn_stats_nchw_kernel(const T* __restrict__ x, double* __restrict
     int64_t chunk = (n_per_g + splits - 1) / splits;
     int64_t lo = blockIdx.y * chunk, hi = min(lo + chunk, n_per_g);
     const T* xg = x + g * n_per_g;
+    const float pv = to_float(xg[0]);
     float s = 0.f, q = 0.f;
-    for (int64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) { float v = to_float(xg[i]); s += v; q += v * v; }
+    for (int64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) { float v = to_float(xg[i]) - pv; s += v; q += v * v; }
     s = block_reduce_sum(s, red);
     q = block_reduce_sum(q, red);
     if (threadIdx.x == 0) { atomicAdd(&stats[2 * g], (double)s); atomicAdd(&stats[2 * g + 1], (double)q); }
@@ -691,6 +707,7 @@ template <typename T, int VEC>
 __global__ void gn_apply_kernel(const T* __restrict__ x, T* __restrict__ y, const double* __restrict__ stats, int nhwc, int64_t C, int64_t HW, int groups,
                                 const T* __restrict__ gamma, const T* __restrict__ beta, float eps, int silu)
 {
+    // stats around the group pivots (gn_mean_var): group g's first element is x[g * cpg] (NHWC) or x[g * cpg * HW] (NCHW)
     osb_pdl_prologue();
     int cpg = (int)(C / groups);
     double inv_n = 1.0 / (double)((int64_t)cpg * HW);
@@ -702,8 +719,8 @@ __global__ void gn_apply_kernel(const T* __restrict__ x, T* __restrict__ y, cons
         for (int k = 0; k < VEC; k++) {
             int64_t c = nhwc ? (int64_t)((e + k) % C) : (int64_t)((e + k) / HW);
             int g = (int)(c / cpg);
-            double meand = stats[2 * g] * inv_n;
-            double vard = stats[2 * g + 1] * inv_n - meand * meand;
+            double meand, vard;
+            gn_mean_var(stats, g, inv_n, to_float(x[(int64_t)g * cpg * (nhwc ? 1 : HW)]), meand, vard);
             float mean = (float)meand;
             float rstd = rsqrtf(fmaxf((float)vard, 0.f) + eps);
             float o = (to_float(v.v[k]) - mean) * rstd;
@@ -1363,8 +1380,8 @@ int osb_group_norm(const void* x, void* y, int dtype, int nhwc, int64_t C, int64
             int64_t ppc2 = (HW + c2 - 1) / c2;
             c2 = (HW + ppc2 - 1) / ppc2;
             const size_t smem2 = sizeof(float) * (2 * groups + (size_t)(256 / (C / vec)) * 2 * C);    // + the per-row partials
-            if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8>), (unsigned)c2, 256, smem2, st, (const __half*)x, stats, (int)C, HW, groups, ppc2, (const __half*)nullptr, (__half*)nullptr);
-            else if (dtype == OSB_F32) osb_launch((gn_stats_nhwc_vec_kernel<float, 4>), (unsigned)c2, 256, smem2, st, (const float*)x, stats, (int)C, HW, groups, ppc2, (const float*)nullptr, (float*)nullptr);
+            if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8>), (unsigned)c2, 256, smem2, st, (const __half*)x, stats, (int)C, HW, groups, ppc2, (const __half*)nullptr, (__half*)nullptr, 1);
+            else if (dtype == OSB_F32) osb_launch((gn_stats_nhwc_vec_kernel<float, 4>), (unsigned)c2, 256, smem2, st, (const float*)x, stats, (int)C, HW, groups, ppc2, (const float*)nullptr, (float*)nullptr, 1);
             else return (int)cudaErrorInvalidValue;
             goto stats_done;
         }
@@ -1432,8 +1449,8 @@ int osb_channel_add_stats(const void* x, const void* addv, void* y, int dtype, i
     int64_t ppc2 = (HW + c2 - 1) / c2;
     c2 = (HW + ppc2 - 1) / ppc2;
     size_t smem = sizeof(float) * (2 * groups + (size_t)rows_per_cta * 2 * C);
-    if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8>), (unsigned)c2, 256, smem, st, (const __half*)x, (double*)stats, (int)C, HW, groups, ppc2, (const __half*)addv, (__half*)y);
-    else osb_launch((gn_stats_nhwc_vec_kernel<float, 4>), (unsigned)c2, 256, smem, st, (const float*)x, (double*)stats, (int)C, HW, groups, ppc2, (const float*)addv, (float*)y);
+    if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8>), (unsigned)c2, 256, smem, st, (const __half*)x, (double*)stats, (int)C, HW, groups, ppc2, (const __half*)addv, (__half*)y, 0);
+    else osb_launch((gn_stats_nhwc_vec_kernel<float, 4>), (unsigned)c2, 256, smem, st, (const float*)x, (double*)stats, (int)C, HW, groups, ppc2, (const float*)addv, (float*)y, 0);
     return launched();
 }
 
