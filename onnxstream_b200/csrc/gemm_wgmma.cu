@@ -779,7 +779,9 @@ int osb_tc_gemm_launch(const void* A, const void* B, void* C, const void* bias, 
     p.C = (__half*)C; p.bias = (const __half*)bias; p.residual = (const __half*)residual; p.stride_c = sc; p.ldc = ldc;
     if (pair) { p.split_k = 1; return launch(ma, mb, p, st, nullptr, nullptr, true); }
     OsbWorkspace* wsp = nullptr;
-    p.split_k = (ldc == N && (sc == M * N || batch == 1)) ? choose_split(p.m_tiles * p.n_tiles * p.batch, p.k_blocks_per_tap, (size_t)batch * M * N, st, &wsp) : 1;
+    // the split-K reduce reads the residual as 8-byte vectors: a residual that is not 8-byte aligned runs unsplit (scalar epilogue reads)
+    const bool split_ok = ldc == N && (sc == M * N || batch == 1) && ((uintptr_t)residual & 7) == 0;
+    p.split_k = split_ok ? choose_split(p.m_tiles * p.n_tiles * p.batch, p.k_blocks_per_tap, (size_t)batch * M * N, st, &wsp) : 1;
     p.ws = wsp ? wsp->splitk : nullptr;
     if (g_f32x && !f32x_params(p, wsp, st)) return (int)cudaErrorNotSupported;
     return launch(ma, mb, p, st);
@@ -865,9 +867,10 @@ int osb_tc_conv_launch(const void* x, const void* w, const void* bias, const voi
         { static const int dbg = env_int("OSB_GN_DEBUG"); p.gn_debug = dbg; }
         return launch(ma, mb, p, st, nullptr, nullptr, true);
     }
-    // the split-K reduce paths move float4 / half4 vectors: ragged Cout (conv_out, 3 or 4 channels) runs unsplit
+    // the split-K reduce paths move float4 / half4 vectors: ragged Cout (conv_out, 3 or 4 channels) and a residual that is not 8-byte
+    // aligned run unsplit
     OsbWorkspace* wsp = nullptr;
-    p.split_k = (Cout % 4 == 0) ? choose_split(p.m_tiles * p.n_tiles, p.taps * p.k_blocks_per_tap, (size_t)Ho * Wo * Cout, st, &wsp) : 1;
+    p.split_k = (Cout % 4 == 0 && ((uintptr_t)residual & 7) == 0) ? choose_split(p.m_tiles * p.n_tiles, p.taps * p.k_blocks_per_tap, (size_t)Ho * Wo * Cout, st, &wsp) : 1;
     p.ws = wsp ? wsp->splitk : nullptr;
     p.bias2 = (const __half*)bias2;
     // statistics: the tile epilogue (unsplit) or the reduce kernel (split-K; needs 4 consecutive columns inside one group)

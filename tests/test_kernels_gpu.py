@@ -1,6 +1,12 @@
 """GPU parity tests for the hand-written kernels, called through the internal C ABI (include/onnxstream_b200_kernels.h)
-with torch only providing device memory.  Reference = fp64 math on the same fp16-rounded inputs; the tolerance for the
-fp16 tensor-core path is |err| <= 2^-9 * sum|a_i b_i| + 1 fp16 ulp of the result (fp32 accumulate, one final rounding)."""
+with torch only providing device memory.  Reference = fp64 math on the same rounded inputs.
+
+Contractions (GEMM, conv, GEMV) are checked in two data regimes (DESIGN.md section 4):
+  * exact: integer-valued operands, bias and residual with S = sum|a_i b_i| + |bias| + |residual| < 2^24 (and every fp16 result below
+    65504).  Every partial sum is then an exact fp32 integer in any summation order, and the one final rounding makes the output equal to
+    the fp64 reference rounded once to the output type, bit for bit (signed zeros aside).
+  * Gaussian: |got - ref| <= 1/2 ulp_out(max(|ref|, |got|)) + 2^-16 * S, i.e. one output rounding plus fp32 accumulation; fp16 accumulation
+    or a lost split plane is far outside it."""
 import ctypes
 
 import numpy as np
@@ -9,6 +15,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 F16, F32 = 2, 3
+ACC_BAR = 2.0 ** -16     # fp32 accumulation, relative to S
 
 
 @pytest.fixture(scope="module")
@@ -32,12 +39,61 @@ def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def _check(out, ref, absref, what):
+def _half_ulp(m, dtype):
+    """1/2 ulp of |values| m (fp64 tensor) in the storage type `dtype` (torch.half / torch.float32), subnormals included."""
     import torch
-    err = (out.double() - ref).abs()
-    tol = absref * 2.0 ** -9 + ref.abs() * 2.0 ** -10 + 1e-6
-    bad = (err > tol)
-    assert not bad.any(), f"{what}: {int(bad.sum())} / {bad.numel()} outside tolerance, max err {float(err.max()):.4g} (ref max {float(ref.abs().max()):.4g})"
+    p, tiny = (11, -14) if dtype == torch.half else (24, -126)
+    e = torch.frexp(m)[1].double()                     # m = f * 2^e, f in [0.5, 1)
+    ulp = torch.where(m < 2.0 ** tiny, torch.full_like(m, 2.0 ** (tiny - p + 1)), torch.pow(2.0, e - p))
+    return 0.5 * ulp
+
+
+def _check(out, ref, absref, what, coef=ACC_BAR):
+    """Gaussian-regime bar: |got - ref| <= 1/2 ulp_out(max(|ref|, |got|)) + coef * S, S = absref = sum|a_i b_i| + |bias| + |residual|.
+    Returns the worst err / bar ratio (printed as '[bar] <path> <ratio>', the path being the first word of `what`)."""
+    import torch
+    got = out.double()
+    err = (got - ref).abs()
+    tol = _half_ulp(torch.maximum(ref.abs(), got.abs()), out.dtype) + coef * absref
+    bad = ~(err <= tol) | ~torch.isfinite(got)
+    ratio = float((err / tol).max())
+    print(f"[bar] {what.split()[0]} {ratio:.4g}")
+    assert not bad.any(), f"{what}: {int(bad.sum())} / {bad.numel()} outside the bar, max err {float(err.max()):.4g}, worst err/bar {ratio:.3g} (ref max {float(ref.abs().max()):.4g})"
+    return ratio
+
+
+def _check_exact(out, ref, absref, what):
+    """Exact regime: integer operands, S < 2^24 -> the output is the fp64 reference rounded once to the output type."""
+    import torch
+    assert float(absref.max()) < 2.0 ** 24, f"{what}: S = {float(absref.max())} leaves the exact range"
+    if out.dtype == torch.half:
+        assert float(ref.abs().max()) < 65504, f"{what}: fp16 overflow in the reference"
+    want = ref.cpu().numpy().astype(np.float16 if out.dtype == torch.half else np.float32)
+    got = out.cpu().numpy()
+    diff = ~(got == want)
+    assert not diff.any(), f"{what}: {int(diff.sum())} / {diff.size} outputs differ from the once-rounded fp64 result, e.g. got {got[diff][:4]} want {want[diff][:4]}"
+
+
+def _operands(regime, g, shapes, dtype, lim=3, row_scaled=0):
+    """Device tensors of `dtype` for each shape: integers in [-lim, lim] (exact regime) or N(0,1), the first `row_scaled` operands with
+    rows of very different scale (Gaussian regime)."""
+    import torch
+    out = []
+    for i, shp in enumerate(shapes):
+        if shp is None:
+            out.append(None)
+        elif regime == "exact":
+            out.append(torch.randint(-lim, lim + 1, shp, device="cuda", generator=g).to(dtype))
+        else:
+            t = torch.randn(shp, device="cuda", generator=g)
+            if i < row_scaled:
+                t = t * torch.exp(torch.randn(shp[:-1] + (1,), device="cuda", generator=g))
+            out.append(t.to(dtype))
+    return out
+
+
+def _verify(regime, out, ref, absref, what):
+    return _check_exact(out, ref, absref, what) if regime == "exact" else _check(out, ref, absref, what)
 
 
 GEMM_CASES = [
@@ -124,26 +180,25 @@ def test_gemm_f16(K, case, impl):
     if impl == 2 and M < 32:
         pytest.skip("skinny problems are served by the weight-bandwidth GEMV kernel, not the tensor-core tile kernel")
     g = torch.Generator(device="cuda").manual_seed(M * 7 + N * 3 + Kd)
-    a = torch.randn(batch, M, Kd, device="cuda", generator=g).half()
-    b = (torch.randn(batch, N, Kd, device="cuda", generator=g) if bt else torch.randn(batch, Kd, N, device="cuda", generator=g)).half()
-    bias = torch.randn(N, device="cuda", generator=g).half() if has_bias else None
-    res = torch.randn(batch, M, N, device="cuda", generator=g).half() if has_res else None
-    c = torch.full((batch, M, N), float("nan"), device="cuda", dtype=torch.half)
-    K.osb_launch_count_reset()
-    rc = K.osb_gemm(a.data_ptr(), b.data_ptr(), c.data_ptr(), bias.data_ptr() if has_bias else None, res.data_ptr() if has_res else None,
-                    batch, M, N, Kd, M * Kd, N * Kd, M * N, bt, F16, impl, _stream())
-    assert rc == 0, f"osb_gemm rc={rc}"
-    torch.cuda.synchronize()
-    if impl == 2:
-        assert K.osb_tc_launch_count() >= 1
-    bd = b.double().transpose(1, 2) if bt else b.double()
-    ref = a.double() @ bd
-    absref = a.double().abs() @ bd.abs()
-    if has_bias:
-        ref = ref + bias.double(); absref = absref + bias.double().abs()
-    if has_res:
-        ref = ref + res.double(); absref = absref + res.double().abs()
-    _check(c, ref, absref, f"gemm {case} impl {impl}")
+    for regime in ("exact", "gauss"):
+        a, b, bias, res = _operands(regime, g, [(batch, M, Kd), (batch, N, Kd) if bt else (batch, Kd, N), (N,) if has_bias else None,
+                                                (batch, M, N) if has_res else None], torch.half, lim=2, row_scaled=1)
+        c = torch.full((batch, M, N), float("nan"), device="cuda", dtype=torch.half)
+        K.osb_launch_count_reset()
+        rc = K.osb_gemm(a.data_ptr(), b.data_ptr(), c.data_ptr(), bias.data_ptr() if has_bias else None, res.data_ptr() if has_res else None,
+                        batch, M, N, Kd, M * Kd, N * Kd, M * N, bt, F16, impl, _stream())
+        assert rc == 0, f"osb_gemm rc={rc}"
+        torch.cuda.synchronize()
+        if impl == 2:
+            assert K.osb_tc_launch_count() >= 1
+        bd = b.double().transpose(1, 2) if bt else b.double()
+        ref = a.double() @ bd
+        absref = a.double().abs() @ bd.abs()
+        if has_bias:
+            ref = ref + bias.double(); absref = absref + bias.double().abs()
+        if has_res:
+            ref = ref + res.double(); absref = absref + res.double().abs()
+        _verify(regime, c, ref, absref, f"gemm_tc {case} impl {impl}" if impl == 2 else f"gemm {case} impl {impl}")
 
 
 CONV_CASES = [
@@ -168,35 +223,75 @@ CONV_CASES = [
     (32, 32, 16, 3, 3, 1, 1, True, False),
     (32, 32, 32, 16, 1, 1, 0, True, True),
     (16, 16, 24, 40, 3, 1, 1, False, False),
+    # kernel / padding geometry: k = (kh, kw), pad = (pad_top, pad_left), applied on both sides
+    (300, 1, 64, 64, (3, 1), 1, (1, 0), True, True),      # Conv1D as op_conv lays it out: H = L, W = 1, kw = 1 (tensor cores: bw = 1, bh = 128)
+    (300, 1, 64, 64, (3, 1), 2, (1, 0), True, False),
+    (300, 1, 64, 64, (5, 1), 1, (2, 0), False, True),
+    (301, 1, 64, 64, (5, 1), 2, (2, 0), True, False),
+    (32, 40, 32, 64, (1, 3), 1, (0, 1), True, False),     # non-square kernels
+    (32, 40, 32, 64, (3, 1), 1, (1, 0), True, True),
+    (24, 40, 32, 64, (1, 7), 1, (0, 3), True, False),
+    (40, 24, 32, 64, (7, 1), 1, (3, 0), False, True),
+    (24, 24, 32, 64, (5, 5), 1, (2, 2), True, False),
+    (64, 64, 16, 64, (7, 7), 2, (3, 3), True, False),     # 7x7 stride-2 stem at Cin = 16: tensor cores
+    (64, 64, 3, 64, (7, 7), 2, (3, 3), True, False),      # ... at Cin = 3: CUDA-core kernel (Cin < 16)
+    (20, 20, 32, 32, 3, 1, (1, 0), True, True),           # pad_top != pad_left
+    (16, 16, 32, 32, 3, 1, 0, True, False),               # 'valid' padding with k > 1
+    (33, 31, 32, 64, 3, 2, 1, True, True),                # odd H / W at stride 2
+    (4, 300, 32, 32, 3, 1, 1, True, False),               # Wo = 300: bw = 128, ragged tiles_x
+    (64, 5, 32, 32, 3, 1, 1, True, True),                 # Wo < 8
+    (16, 16, 16, 24, (9, 9), 1, (4, 4), True, False),     # kh > 7: CUDA-core kernel
+    (7, 7, 32, 32, 3, 1, 1, True, True),                  # H * W < 64: CUDA-core kernel
 ]
+
+
+def _conv_geom(case):
+    H, W, Cin, Cout, k, s, pad, has_bias, has_res = case
+    kh, kw = k if isinstance(k, tuple) else (k, k)
+    pt, pl = pad if isinstance(pad, tuple) else (pad, pad)
+    return H, W, Cin, Cout, kh, kw, s, pt, pl, has_bias, has_res
 
 
 @pytest.mark.parametrize("case", CONV_CASES)
 @pytest.mark.parametrize("impl", [1, 0])
 def test_conv_f16(K, case, impl):
+    """impl 1: igemm_kernel (CUDA cores).  impl 0: the tensor cores exactly when osb_conv2d_fusable says so (fp16, Cin % 8 == 0, Cin >= 16,
+    H * W >= 64, kh, kw <= 7, stride <= 2, 16-byte pointers, Cout % 8 == 0), else igemm_kernel -- asserted through the launch counters."""
     import torch
     import torch.nn.functional as Fn
-    H, W, Cin, Cout, k, s, pad, has_bias, has_res = case
+    H, W, Cin, Cout, kh, kw, s, pt, pl, has_bias, has_res = _conv_geom(case)
+    vp, i64, ci = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int
+    K.osb_conv2d_fusable.argtypes = [vp, vp, vp, i64, i64, i64, i64, ci, ci, ci, ci, ci]
     g = torch.Generator(device="cuda").manual_seed(H * 5 + Cin)
-    x = torch.randn(H, W, Cin, device="cuda", generator=g).half()
-    w = (torch.randn(Cout, k, k, Cin, device="cuda", generator=g) / (k * k * Cin) ** 0.5).half()
-    bias = torch.randn(Cout, device="cuda", generator=g).half() if has_bias else None
-    Ho, Wo = (H + 2 * pad - k) // s + 1, (W + 2 * pad - k) // s + 1
-    res = torch.randn(Ho, Wo, Cout, device="cuda", generator=g).half() if has_res else None
-    y = torch.full((Ho, Wo, Cout), float("nan"), device="cuda", dtype=torch.half)
-    rc = K.osb_conv2d(x.data_ptr(), w.data_ptr(), bias.data_ptr() if has_bias else None, res.data_ptr() if has_res else None, y.data_ptr(),
-                      H, W, Cin, Cout, k, k, s, pad, pad, Ho, Wo, F16, impl, _stream())
-    assert rc == 0, f"osb_conv2d rc={rc}"
-    torch.cuda.synchronize()
-    xn = x.double().permute(2, 0, 1)[None]
-    wn = w.double().permute(0, 3, 1, 2)
-    ref = Fn.conv2d(xn, wn, None, stride=s, padding=pad)[0].permute(1, 2, 0)
-    absref = Fn.conv2d(xn.abs(), wn.abs(), None, stride=s, padding=pad)[0].permute(1, 2, 0)
-    if has_bias:
-        ref = ref + bias.double(); absref = absref + bias.double().abs()
-    if has_res:
-        ref = ref + res.double(); absref = absref + res.double().abs()
-    _check(y, ref, absref, f"conv {case} impl {impl}")
+    Ho, Wo = (H + 2 * pt - kh) // s + 1, (W + 2 * pl - kw) // s + 1
+    for regime in ("exact", "gauss"):
+        x, w, bias, res = _operands(regime, g, [(H, W, Cin), (Cout, kh, kw, Cin), (Cout,) if has_bias else None, (Ho, Wo, Cout) if has_res else None],
+                                    torch.float32, lim=3)
+        if regime == "gauss":
+            w = w / (kh * kw * Cin) ** 0.5
+        x, w = x.half(), w.half()
+        bias = bias.half() if has_bias else None
+        res = res.half() if has_res else None
+        y = torch.full((Ho, Wo, Cout), float("nan"), device="cuda", dtype=torch.half)
+        K.osb_launch_count_reset()
+        rc = K.osb_conv2d(x.data_ptr(), w.data_ptr(), bias.data_ptr() if has_bias else None, res.data_ptr() if has_res else None, y.data_ptr(),
+                          H, W, Cin, Cout, kh, kw, s, pt, pl, Ho, Wo, F16, impl, _stream())
+        assert rc == 0, f"osb_conv2d rc={rc}"
+        torch.cuda.synchronize()
+        on_tc = impl != 1 and K.osb_conv2d_fusable(x.data_ptr(), w.data_ptr(), y.data_ptr(), H, W, Cin, Cout, kh, kw, s, F16, impl) == 1
+        if impl == 1 or Cout % 8 == 0:
+            assert (K.osb_tc_launch_count() >= 1) == on_tc, f"expected the {'tensor-core' if on_tc else 'CUDA-core'} path"
+        else:       # ragged Cout (conv_out): not fusable (no bias2 / statistics), yet the plain conv runs on the tensor cores with a scalar epilogue
+            on_tc = K.osb_tc_launch_count() >= 1
+        xn = x.double().permute(2, 0, 1)[None]
+        wn = w.double().permute(0, 3, 1, 2)
+        ref = Fn.conv2d(xn, wn, None, stride=s, padding=(pt, pl))[0].permute(1, 2, 0)
+        absref = Fn.conv2d(xn.abs(), wn.abs(), None, stride=s, padding=(pt, pl))[0].permute(1, 2, 0)
+        if has_bias:
+            ref = ref + bias.double(); absref = absref + bias.double().abs()
+        if has_res:
+            ref = ref + res.double(); absref = absref + res.double().abs()
+        _verify(regime, y, ref, absref, f"{'conv_tc' if on_tc else 'conv_igemm'} {case} impl {impl}")
 
 
 GN_CONV_CASES = [
