@@ -199,6 +199,16 @@ int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype);
 int osb_flash_attention(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
                         int64_t heads, int64_t T, int64_t Tk, int64_t d, float scale, void* stream);
 
+/* Fused flash-style attention on wgmma for wide heads (fp16, 160 < d <= 512, d % 8 == 0): the VAE decoder's single-head d = 512
+ * self-attention, the AttentionFusedOps branch (src/onnxstream.cpp:6696-6929) without its [Tq, Tk] score buffer.  q [h,T,d], k [h,d,Tk]
+ * when k_transposed (Tk % 8 == 0) else [h,Tk,d], v [h,Tk,d], out [h,T,d]; contiguous, 16-byte aligned.  No scratch: memory is the
+ * operands and the output.  *_ok: the shape and dtype; the launch returns cudaErrorInvalidValue (and launches nothing) for anything
+ * *_ok refuses, for misaligned pointers, for a transposed K whose rows are not a multiple of 16 bytes (transpose it to [h,Tk,d] first)
+ * and for scale <= 0. */
+int osb_flash_attention_wide_ok(int64_t T, int64_t Tk, int64_t d, int dtype);
+int osb_flash_attention_wide(const void* q, const void* k, const void* v, void* out, int64_t heads, int64_t T, int64_t Tk, int64_t d,
+                             float scale, int k_transposed, int dtype, void* stream);
+
 /* Fused flash-style ScaledDotProductAttention on wgmma (fp16; d % 8 == 0, 8 <= d <= 128, dv == d): the prefill case of
  * src/onnxstream.cpp:7767-7882.  Semantics of osb_attention with k_transposed = 0: q [Hq,Tq,d], k / v [Hkv,Tk,d], additive mask
  * [Tq,Tk] (optional), out [Hq,Tq,d]; query head h reads KV head h / (Hq / Hkv).  The Hq / Hkv query heads of one KV head are

@@ -16,6 +16,7 @@
 //
 // sdpa_flash_kernel (below): the unpipelined structure for ScaledDotProductAttention with grouped KV heads and an additive mask --
 // llm.cpp's prompt prefill -- for d <= 128.
+// flash_attention_wide_kernel (below): 160 < d <= 512 -- the VAE decoder's single-head d = 512 attention -- with O split over its columns.
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -619,6 +620,227 @@ int fa_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void
     return launched(1);
 }
 
+// ---- wide heads: 160 < d <= 512 (the VAE's single-head d = 512 attention) --------------------------------------------------------------
+// softmax(Q K^T * scale) V for q [h, T, d], k [h, Tk, d] (KT = false) or [h, d, Tk] (KT = true), v [h, Tk, d], out [h, T, d].
+// A 64-row x 512-column fp32 O would take 256 registers per consumer thread, so O is split over its columns: one CTA per (256-column slice
+// of V and O, 64-query tile, head).  Each CTA computes the full S = Q K^T over d in 64-column chunks and then O_slice += P V_slice, so
+// Q K^T runs once per slice: at d = 512 the two slices make 2 + 1 = 3 units of MMA work where the unsplit product has 2.  Slices of the
+// same query tile are adjacent in the grid, so their K / V tiles are read from HBM once and from L2 by the sibling.
+// 256 threads: warpgroup 0 is the TMA producer (one warp, 40 registers), warpgroup 1 takes the 64 query rows (240 registers: O 128 + S 32
+// + P 16).  With two consumer warpgroups (384 threads) ptxas allocates at most 168 registers per thread: a 256-column O spills and
+// 128-column slices would make Q K^T 4 + 1 = 5 units of MMA work at d = 512.  Q stays in shared memory (up to 8 chunks, 64 KB); K streams
+// through a ring of 64-column chunks of one 64-key tile (a chunk is released as soon as the MMAs that read it retire), V through a ring of
+// 64-key x 256-column tiles.  The consumer loop is not software-pipelined (Q K^T is 2/3 of the MMA work).  Numerics are those of
+// flash_attention_kernel with the exact running maximum.
+constexpr int WD_BQ = 64;                 // queries per CTA: one consumer warpgroup
+constexpr int WD_BK = 64;                 // keys per tile
+constexpr int WD_NV = 4;                  // 64-column chunks of V / O per CTA
+constexpr int WD_DCH = 8;                 // largest number of 64-column chunks of d
+constexpr int WD_K_STAGES = 8, WD_V_STAGES = 2;
+constexpr int WD_THREADS = 256, WD_CONSUMERS = 128;
+constexpr int WD_PRODUCER_REGS = 40, WD_CONSUMER_REGS = 240;
+constexpr int WD_Q_CHUNK = WD_BQ * 128;   // 64 rows x 64 fp16 columns
+constexpr int WD_K_CHUNK = WD_BK * 128;   // 64 keys x 64 columns of d (or 64 rows of d x 64 keys)
+constexpr int WD_V_CHUNK = WD_BK * 128;
+constexpr int WD_V_BYTES = WD_NV * WD_V_CHUNK;
+constexpr int WD_SMEM = WD_DCH * WD_Q_CHUNK + WD_K_STAGES * WD_K_CHUNK + WD_V_STAGES * WD_V_BYTES + 1024 + 256;
+
+// S (+)= Q_c K_c^T for one 64-column chunk c of d: 4 k-steps.  K-major K: 32 B per k-step inside the swizzle row; MN-major K^T (rows of
+// d): 16 rows of d = 2048 B per k-step.
+template <bool KT>
+__device__ __forceinline__ void wd_issue_qk_chunk(float (&s)[WD_BK / 2], uint64_t qdesc, uint64_t kdesc, bool first)
+{
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        wgmma_m64n64k16_f16<KT ? 1 : 0>(s, qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(KT ? (k * 2048) >> 4 : k * 2), (first && k == 0) ? 0u : 1u);
+    wgmma_commit();
+}
+
+// O_slice += P V_slice for one key tile, one wgmma group: 64-column chunks of V WD_V_CHUNK bytes apart, MN-major, 16 keys = 2048 B per
+// k-step.  Chunks wholly past d (d <= 192, or the last slice) are not loaded: their MMAs read stale shared memory into output columns
+// that are never stored.
+__device__ __forceinline__ void wd_issue_pv(float (&o)[WD_NV][32], uint32_t (&a)[WD_BK / 16][4], uint64_t vdesc)
+{
+#pragma unroll
+    for (int ch = 0; ch < WD_NV; ch++) fence_regs(o[ch]);
+    fence_regs(a);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < WD_BK / 16; kk++)
+#pragma unroll
+        for (int ch = 0; ch < WD_NV; ch++)
+            wgmma_m64n64k16_f16_rs(o[ch], a[kk], vdesc + (uint64_t)((ch * WD_V_CHUNK + kk * 2048) >> 4), 1u);
+    wgmma_commit();
+}
+
+template <bool KT>
+__global__ void __launch_bounds__(WD_THREADS, 1)
+flash_attention_wide_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+                            const __grid_constant__ CUtensorMap map_v, const FaParams p)
+{
+    constexpr int KS = WD_K_STAGES, VS = WD_V_STAGES;
+    osb_pdl_trigger_entry();
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint8_t* sQ = smem;
+    uint8_t* sK = sQ + WD_DCH * WD_Q_CHUNK;
+    uint8_t* sV = sK + KS * WD_K_CHUNK;
+    uint64_t* bars = (uint64_t*)(sV + VS * WD_V_BYTES);
+    uint64_t* q_full = bars;                           // [1]
+    uint64_t* k_full = bars + 1;                       // [KS]
+    uint64_t* k_empty = k_full + KS;                   // [KS]: one arrival per consumer warp
+    uint64_t* v_full = k_empty + KS;                   // [VS]
+    uint64_t* v_empty = v_full + VS;                   // [VS]
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    // blockIdx.x = query tile * slices + slice: the slices of one query tile are adjacent, and x takes any T (y would stop at 65535 tiles)
+    const int n_slices = (p.d + 64 * WD_NV - 1) / (64 * WD_NV);
+    const int col0 = (blockIdx.x % n_slices) * (64 * WD_NV);
+    const int q0 = (blockIdx.x / n_slices) * WD_BQ;
+    const int head = blockIdx.y;
+    const int n_dch = (p.d + 63) >> 6;
+
+    if (warp == 0 && lane == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
+    }
+    if (warp == 1 && lane == 0) {
+        mbar_init(q_full, 1);
+        for (int i = 0; i < KS; i++) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], WD_CONSUMERS / 32); }
+        for (int i = 0; i < VS; i++) { mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], WD_CONSUMERS / 32); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    osb_pdl_wait();
+
+    const int n_kv = p.kv_tiles;
+
+    if (warp < 4) {
+        setmaxnreg_dec<WD_PRODUCER_REGS>();
+        if (warp == 0) {
+            if (elect_one()) {
+                mbar_expect_tx(q_full, n_dch * WD_Q_CHUNK);
+                for (int c = 0; c < n_dch; c++) tma_load_3d(sQ + c * WD_Q_CHUNK, &map_q, q_full, 64 * c, q0, head);
+            }
+            __syncwarp();
+            // V chunks wholly past d are not loaded: they only feed output columns that are never stored
+            const int n_vch = min(WD_NV, (p.d - col0 + 63) >> 6);
+            int kc = 0;
+            for (int j = 0; j < n_kv; j++) {
+                for (int c = 0; c < n_dch; c++, kc++) {
+                    const int st = kc % KS;
+                    mbar_wait(&k_empty[st], ((kc / KS) & 1) ^ 1);
+                    if (elect_one()) {
+                        mbar_expect_tx(&k_full[st], WD_K_CHUNK);
+                        if (KT) tma_load_3d(sK + st * WD_K_CHUNK, &map_k, &k_full[st], j * WD_BK, 64 * c, head);
+                        else tma_load_3d(sK + st * WD_K_CHUNK, &map_k, &k_full[st], 64 * c, j * WD_BK, head);
+                    }
+                    __syncwarp();
+                }
+                const int sv = j % VS;
+                mbar_wait(&v_empty[sv], ((j / VS) & 1) ^ 1);
+                if (elect_one()) {
+                    mbar_expect_tx(&v_full[sv], n_vch * WD_V_CHUNK);
+                    for (int ch = 0; ch < n_vch; ch++)
+                        tma_load_3d(sV + sv * WD_V_BYTES + ch * WD_V_CHUNK, &map_v, &v_full[sv], col0 + 64 * ch, j * WD_BK, head);
+                }
+                __syncwarp();
+            }
+        }
+    } else {
+        // ===================== warpgroup 1: the CTA's 64 query rows =====================
+        setmaxnreg_inc<WD_CONSUMER_REGS>();
+        const int r = (warp & 3) * 16 + (lane >> 2);
+        const int cq = 2 * (lane & 3);
+        // Q K-major (8-row groups 1024 B apart); K K-major or K^T MN-major and V MN-major, 8-row groups 1024 B apart
+        const uint64_t qdesc0 = make_smem_desc(smem_u32(sQ), 16, 1024);
+        const uint64_t kdesc0 = make_smem_desc(smem_u32(sK), KT ? WD_K_CHUNK : 16, 1024);
+        const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), WD_V_CHUNK, 1024);
+        float o[WD_NV][32];
+#pragma unroll
+        for (int ch = 0; ch < WD_NV; ch++)
+#pragma unroll
+            for (int i = 0; i < 32; i++) o[ch][i] = 0.f;
+        float s[WD_BK / 2];
+        uint32_t a[WD_BK / 16][4];
+        float m_run[2] = { -INFINITY, -INFINITY }, l_run[2] = { 0.f, 0.f }, alpha[2];
+        mbar_wait(q_full, 0);
+        int kc = 0;
+        for (int j = 0; j < n_kv; j++) {
+            // S = Q K_j^T, one wgmma group per chunk of d; a chunk's slot is released once the next chunk's group is issued and it retired
+            fence_regs(s);
+            for (int c = 0; c < n_dch; c++, kc++) {
+                const int st = kc % KS;
+                mbar_wait(&k_full[st], (kc / KS) & 1);
+                wgmma_fence();
+                wd_issue_qk_chunk<KT>(s, qdesc0 + (uint64_t)((c * WD_Q_CHUNK) >> 4), kdesc0 + (uint64_t)((st * WD_K_CHUNK) >> 4), c == 0);
+                if (c > 0) {
+                    wgmma_wait<1>();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&k_empty[(kc - 1) % KS]);
+                }
+            }
+            wgmma_wait<0>();
+            fence_regs(s);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&k_empty[(kc - 1) % KS]);
+            fa_softmax<WD_BK>(s, m_run, l_run, alpha, j * WD_BK, cq, p);
+            fa_rescale_pack<WD_NV, WD_BK>(o, a, s, alpha);
+            // O_slice += P V_slice
+            const int sv = j % VS;
+            mbar_wait(&v_full[sv], (j / VS) & 1);
+            wd_issue_pv(o, a, vdesc0 + (uint64_t)((sv * WD_V_BYTES) >> 4));
+            wgmma_wait<0>();
+#pragma unroll
+            for (int ch = 0; ch < WD_NV; ch++) fence_regs(o[ch]);
+            fence_regs(a);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&v_empty[sv]);
+        }
+        // epilogue: O / l -> fp16 -> out[head][q][col0 + c]
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            float l = l_run[h];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = 1.f / l;
+            const int qrow = q0 + r + 8 * h;
+            if (qrow >= p.T) continue;
+            __half* orow = p.out + ((long long)head * p.T + qrow) * p.ldo + col0;
+#pragma unroll
+            for (int ch = 0; ch < WD_NV; ch++)
+#pragma unroll
+                for (int c = 0; c < 8; c++) {
+                    const int col = 64 * ch + 8 * c + cq;
+                    if (col0 + col < p.d)     // d % 8 == 0: the pair is inside
+                        *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
+                }
+        }
+    }
+}
+
+template <bool KT>
+int wd_launch(const void* q, const void* k, const void* v, const FaParams& p, int64_t heads, cudaStream_t st)
+{
+    // q / v / out [heads, rows, d] viewed as (d, rows, heads); K^T [heads, d, Tk] as (Tk, d, heads) with 64 x 64 boxes
+    CUtensorMap mq, mk, mv;
+    const bool ok_k = KT ? sdpa_map(&mk, k, p.Tk, p.d, heads, 64) : sdpa_map(&mk, k, p.d, p.Tk, heads, WD_BK);
+    if (!sdpa_map(&mq, q, p.d, p.T, heads, WD_BQ) || !ok_k || !sdpa_map(&mv, v, p.d, p.Tk, heads, WD_BK)) return (int)cudaErrorInvalidValue;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(flash_attention_wide_kernel<KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, WD_SMEM);
+        if (e != cudaSuccess) return (int)e;
+        attr = true;
+    }
+    FaParams pp = p;
+    pp.kv_tiles = (p.Tk + WD_BK - 1) / WD_BK;
+    const int64_t n_slices = (p.d + 64 * WD_NV - 1) / (64 * WD_NV);
+    dim3 grid((unsigned)((p.T + WD_BQ - 1) / WD_BQ * n_slices), (unsigned)heads);
+    osb_launch((flash_attention_wide_kernel<KT>), grid, WD_THREADS, (size_t)WD_SMEM, st, mq, mk, mv, pp);
+    return launched(1);
+}
+
 }  // namespace
 
 extern "C" int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
@@ -645,6 +867,30 @@ extern "C" int osb_flash_attention(const void* q, int64_t ldq, const void* k, in
     if (d <= 80) return fa_launch<2, 64, 5>(q, ldq, k, ldk, v, ldv, p, heads, st);
     if (d <= 128) return fa_launch<2, 64, 8>(q, ldq, k, ldk, v, ldv, p, heads, st);
     return fa_launch<3, 32, 10>(q, ldq, k, ldk, v, ldv, p, heads, st);
+}
+
+extern "C" int osb_flash_attention_wide_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
+{
+    return dtype == OSB_F16 && d > 160 && d <= 64 * WD_DCH && d % 8 == 0 && T >= 1 && Tk >= 1 && T <= (int64_t)INT32_MAX - WD_BQ &&
+           Tk <= (int64_t)INT32_MAX - WD_BK && fa_encode() != nullptr;
+}
+
+// q [h, T, d], k [h, Tk, d] or (k_transposed) [h, d, Tk], v [h, Tk, d], out [h, T, d]; fp16, contiguous, 16-byte aligned.  K^T rows are
+// Tk elements long, so k_transposed needs Tk % 8 == 0 (TMA row strides are multiples of 16 bytes).  scale > 0: the running maximum is
+// taken over the raw scores.
+extern "C" int osb_flash_attention_wide(const void* q, const void* k, const void* v, void* out, int64_t heads, int64_t T, int64_t Tk, int64_t d,
+                                        float scale, int k_transposed, int dtype, void* stream)
+{
+    if (!osb_flash_attention_wide_ok(T, Tk, d, dtype) || heads < 1 || heads > 65535 || (k_transposed && Tk % 8) || !(scale > 0.f) || !(scale < INFINITY))
+        return (int)cudaErrorInvalidValue;
+    if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) != 0) return (int)cudaErrorInvalidValue;
+    FaParams p{};
+    p.T = (int)T; p.Tk = (int)Tk; p.d = (int)d;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    p.tau = 0.f;
+    p.out = (__half*)out; p.ldo = d;
+    cudaStream_t st = (cudaStream_t)stream;
+    return k_transposed ? wd_launch<true>(q, k, v, p, heads, st) : wd_launch<false>(q, k, v, p, heads, st);
 }
 
 extern "C" int osb_sdpa_flash_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, int dtype)

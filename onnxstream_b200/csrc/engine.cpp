@@ -184,8 +184,8 @@ void DevicePool::add_slab(size_t min_bytes)
     check_cuda(cudaMalloc(&p, bytes), "DevicePool cudaMalloc");
     m_slabs.push_back({ p, bytes });
     m_reserved += bytes;
+    m_in_use += bytes;  // release() subtracts (clamped at zero: adding after it would count the slab as in use whenever it exceeds m_in_use)
     release(p, bytes);
-    m_in_use += bytes;  // release() subtracts
 }
 
 DevPtr DevicePool::alloc(size_t bytes)

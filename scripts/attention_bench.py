@@ -12,6 +12,15 @@ Prints ONE JSON line: the card (name, power limit, max SM clock, read with an nv
           per SM, 132 SMs, the card's max SM clock) and MMA (the data sheet's 989 TFLOP/s dense fp16 on the padded shapes the kernel
           runs: keys rounded up to its key tile, QK^T contracted over its k-steps of 16, PV n = d rounded up to 64; FLASH_TILES).
           max|flash - chain| on the same inputs.
+  vae   : (--vae, instead of kernel) the VAE decoder's mid-block attention, one head at d = 512 with K pre-transposed [d, Tk] as the
+          graph has it, at T = Tk = 1024 (32^2 latent) ... 4096 (64^2) and 16384 (128^2), ms per call for
+            flash  : osb_flash_attention_wide
+            chain  : attention_core's chain: osb_gemm(QK^T) -> osb_softmax_scaled -> osb_gemm(PV) through an fp16 [T, Tk] buffer
+          TFLOP/s as 4*T*Tk*d / t; flash_mma_tflops counts the MMA work the kernel issues (Q K^T once per 256-column slice of V, so
+          2*T*Tk*d*(slices + 1)); the score buffer the chain allocates; max|flash - chain|.
+          tiled: the SD VAE decoder (emit.VAEConfig(), 32 x 32 latent tiles: T = 1024 per tile, the shape where the kernel alone is
+          slower than the chain) decoding a 64 x 64 latent as 9 batch siblings of one run (tiled_vae.py), b200_flash_attention on and
+          off alternated; device ms per run (last_gpu_ms), median of --tiled-runs runs after 2 warm-up runs each.
   trace : (--trace DIR) per-kernel-name GPU time of one eager SD 1.5 UNet step (64x64 latent, fp16, resident weights, no CUDA graph)
           and the attention share: flash_attention_kernel, softmax_scaled_* and the tensor-core GEMM launched right before and right
           after each softmax (the QK^T / PV pair) over all kernel and memset time.  The chrome trace is written to DIR.
@@ -114,6 +123,93 @@ def kernel_level(iters, warmup, clock_hz):
     return out
 
 
+VAE_SHAPES = [("vae_32sq", 1024), ("vae_40sq", 1600), ("vae_48sq", 2304), ("vae_56sq", 3136), ("vae_64sq", 4096), ("vae_128sq", 16384)]
+
+
+def vae_level(iters, warmup):
+    import torch
+    lib = ctypes.CDLL(ENGINE_LIB)
+    vp, i64, cf, ci = ctypes.c_void_p, ctypes.c_int64, ctypes.c_float, ctypes.c_int
+    lib.osb_flash_attention_wide.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64, cf, ci, ci, vp]
+    lib.osb_gemm.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i64, i64, i64, i64, ci, ci, ci, vp]
+    lib.osb_softmax_scaled.argtypes = [vp, vp, ci, i64, i64, cf, vp, i64, vp]
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    d, out = 512, []
+    for name, T in VAE_SHAPES:
+        Tk = T
+        g = torch.Generator(device="cuda").manual_seed(T + d)
+        q = torch.randn(T, d, device="cuda", generator=g).half()
+        kt = torch.randn(d, Tk, device="cuda", generator=g).half()
+        v = torch.randn(Tk, d, device="cuda", generator=g).half()
+        S = torch.empty(T, Tk, device="cuda", dtype=torch.half)
+        o_flash = torch.zeros(T, d, device="cuda", dtype=torch.half)
+        o_chain = torch.zeros(T, d, device="cuda", dtype=torch.half)
+        scale = float(torch.tensor(1.0 / d ** 0.5).half())
+
+        def flash():
+            assert lib.osb_flash_attention_wide(q.data_ptr(), kt.data_ptr(), v.data_ptr(), o_flash.data_ptr(), 1, T, Tk, d, scale, 1, F16, stream) == 0
+
+        def chain():
+            assert lib.osb_gemm(q.data_ptr(), kt.data_ptr(), S.data_ptr(), None, None, 1, T, Tk, d, T * d, Tk * d, T * Tk, 0, F16, 0, stream) == 0
+            assert lib.osb_softmax_scaled(S.data_ptr(), S.data_ptr(), F16, T, Tk, scale, None, T, stream) == 0
+            assert lib.osb_gemm(S.data_ptr(), v.data_ptr(), o_chain.data_ptr(), None, None, 1, T, d, Tk, T * Tk, Tk * d, T * d, 0, F16, 0, stream) == 0
+
+        def timed(fn):
+            for _ in range(warmup):
+                fn()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(iters):
+                fn()
+            e1.record()
+            torch.cuda.synchronize()
+            return e0.elapsed_time(e1) / iters
+
+        t_flash, t_chain = timed(flash), timed(chain)
+        flop = 4.0 * T * Tk * d
+        slices = -(-d // 256)
+        out.append({"shape": name, "h": 1, "T": T, "Tk": Tk, "d": d, "flash_ms": round(t_flash, 4), "chain_ms": round(t_chain, 4),
+                    "flash_tflops": round(flop / t_flash / 1e9, 2), "chain_tflops": round(flop / t_chain / 1e9, 2),
+                    "flash_mma_tflops": round(2.0 * T * Tk * d * (slices + 1) / t_flash / 1e9, 2), "flash_vs_chain": round(t_chain / t_flash, 2),
+                    "chain_score_bytes": T * Tk * 2, "max_abs_diff": float((o_flash.float() - o_chain.float()).abs().max())})
+        del q, kt, v, S, o_flash, o_chain
+        torch.cuda.empty_cache()
+    return out
+
+
+def tiled_level(runs):
+    import numpy as np
+    from onnxstream_b200 import tiled_vae as tv
+    d = tempfile.mkdtemp(prefix="osb200_attn_tiled_") + "/"
+    try:
+        emit.emit_vae_decoder(d, emit.VAEConfig(latent=32), "float16")
+        latent = np.random.default_rng(0).standard_normal((1, 4, 64, 64)).astype(np.float32)
+        models = {}
+        for flash in (1, 0):
+            m = Model(ENGINE_LIB, 0, "ram+nocache")
+            for o in ("use_fp16_arithmetic", "fuse_ops_in_attention"):
+                m.set_option(o, True)
+            m.lib.model_set_option(m.h, b"b200_resident_weights", 1)
+            m.lib.model_set_option(m.h, b"b200_flash_attention", flash)
+            m.read_file(d + "model.txt")
+            models[flash] = m
+        ms, imgs, tiles = {1: [], 0: []}, {}, 0
+        for i in range(runs + 2):
+            for flash in (1, 0):
+                imgs[flash], tiles = tv.tiled_decode(models[flash], latent, "input_2E_1", "outsample")
+                if i >= 2:
+                    ms[flash].append(models[flash].stats()["last_gpu_ms"])
+        launches = {f: int(models[f].stats()["kernel_launches"]) for f in (1, 0)}
+        for m in models.values():
+            m.close()
+    finally:
+        shutil.rmtree(d, ignore_errors=True)
+    med = {f: float(np.median(v)) for f, v in ms.items()}
+    return {"tiles": tiles, "tile_T": 1024, "flash_ms": round(med[1], 3), "chain_ms": round(med[0], 3), "flash_runs_ms": [round(x, 3) for x in ms[1]],
+            "chain_runs_ms": [round(x, 3) for x in ms[0]], "launches_flash": launches[1], "launches_chain": launches[0],
+            "max_abs_diff": float(np.abs(imgs[1] - imgs[0]).max())}
+
+
 def trace_step(trace_dir):
     """One eager SD 1.5 UNet step under torch.profiler (CUDA activities); per-kernel GPU time and attention's share of it."""
     import torch
@@ -197,13 +293,19 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--trace", default=None, metavar="DIR", help="also trace one eager UNet step and write the chrome trace to DIR")
     ap.add_argument("--skip-kernels", action="store_true")
+    ap.add_argument("--vae", action="store_true", help="time the VAE's d = 512 attention shapes instead of the UNet's")
+    ap.add_argument("--tiled-runs", type=int, default=7, help="--vae: timed tiled decodes per setting (0 = skip)")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         sys.exit("attention_bench.py needs a CUDA device")
     c = card()
     res = {"card": c, "engine_lib": os.path.basename(ENGINE_LIB)}
-    if not a.skip_kernels:
+    if a.vae:
+        res["vae"] = vae_level(a.iters, a.warmup)
+        if a.tiled_runs:
+            res["tiled"] = tiled_level(a.tiled_runs)
+    elif not a.skip_kernels:
         res["kernel"] = kernel_level(a.iters, a.warmup, float(c["max_sm_clock"].split()[0]) * 1e6)
     if a.trace:
         res["trace"] = trace_step(a.trace)
