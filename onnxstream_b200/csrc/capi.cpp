@@ -6,6 +6,7 @@
 // exceptions thrown across the boundary (model_run, model_set_option, model_add_tensor) exactly where the reference
 // throws them.
 #include "engine_impl.h"
+#include "plan.h"
 #include "../../include/onnxstream_b200.h"
 
 #include <cuda_profiler_api.h>
@@ -264,7 +265,7 @@ char* model_b200_plan_summary(const char* model_text, int fp16_arithmetic, int f
 {
     std::string r;
     try {
-        r = osb::Engine::plan_summary(model_text ? model_text : "", fp16_arithmetic != 0, fuse_nodes != 0, fuse_attention != 0, use_scaled_dp_attn_op != 0);
+        r = osb::plan_summary(model_text ? model_text : "", fp16_arithmetic != 0, fuse_nodes != 0, fuse_attention != 0, use_scaled_dp_attn_op != 0);
     } catch (const std::exception& e) {
         r = std::string("=== ERROR === ") + e.what();
     }

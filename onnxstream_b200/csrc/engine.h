@@ -103,6 +103,8 @@ struct OpDef {                        // src/onnxstream.h:253-264
     const std::string* attr(const char* key) const;
 };
 
+std::vector<OpDef> parse_model_text(const std::string& text, bool dynamic_shapes);
+
 // ---- weights -------------------------------------------------------------------------------------------------
 // Host-side source of weight bytes.  Mirrors the WeightsProvider contract (src/onnxstream.h:266-291): `on_init` once
 // per weight in graph order, `on_restart` at the start of every later run, `fetch` synchronously in graph order.
@@ -160,16 +162,10 @@ struct HostTensor {                   // what is left in the model's tensor list
     int64_t* i64() const { return (int64_t*)buf->ptr; }
 };
 
-struct EngineNoDevice {};   // tag: construct the host-side planner only
-
 class Engine {
 public:
-    explicit Engine(EngineNoDevice);
     explicit Engine(int device = -1);
     ~Engine();
-    // Host-only planning (no CUDA device needed): parse `model_text`, run the fusion matchers, return one line per execution step
-    // ("KIND ops first_op_type first_op_name") followed by a "#summary" line.  Used by the CPU test-suite to pin the planner.
-    static std::string plan_summary(const std::string& model_text, bool fp16_arithmetic, bool fuse_nodes, bool fuse_attention, bool use_sdpa_rewrite = false);
 
     // --- the reference's public knobs (src/onnxstream.h:944-968) ---
     bool use_fp16_arithmetic = false;
@@ -234,7 +230,6 @@ public:
     CUstream_st* compute_stream() const { return m_stream; }
 
 private:
-    friend struct OpCtx;
     int m_device = 0;
     CUstream_st* m_stream = nullptr;
     std::string m_text, m_path;
@@ -255,7 +250,6 @@ private:
     void parse();
     void invalidate_plan();
     std::string options_signature() const;
-    void run_body(bool capturing);
     bool try_replay();
     void drop_graph();
     struct Impl;

@@ -11,8 +11,6 @@
 
 namespace osb {
 
-std::vector<OpDef> parse_model_text(const std::string& text, bool dynamic_shapes);
-
 // Pinned host -> HBM ring on a side stream.  One slot per streamed weight blob; slots are FIFO in graph order.
 class WeightStreamer {
 public:
