@@ -199,6 +199,16 @@ int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype);
 int osb_flash_attention(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
                         int64_t heads, int64_t T, int64_t Tk, int64_t d, float scale, void* stream);
 
+/* osb_flash_attention for fp32 (8 <= d <= 160, d % 8 == 0) on the bf16 tensor cores at fp32 accuracy: q, k and v are split into three
+ * bf16 planes each (the triple split of osb_tc_gemm_f32x), Q K^T and P V sum the six significant cross products in fp32, the softmax is
+ * fp32 with an exact running maximum.  Same layouts as osb_flash_attention with fp32 elements; row strides are multiples of 4 elements and
+ * at least heads * d, pointers 16-byte aligned.  `planes`: device scratch of 6 * (T + 2 * Tk) * heads * d bytes (16-byte aligned) for the
+ * bf16 planes, written by the launch.  The launch returns cudaErrorInvalidValue and enqueues nothing for anything *_ok refuses, for
+ * misaligned pointers or strides and for scale <= 0. */
+int osb_flash_attention_f32x_ok(int64_t T, int64_t Tk, int64_t d, int dtype);
+int osb_flash_attention_f32x(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
+                             int64_t heads, int64_t T, int64_t Tk, int64_t d, float scale, void* planes, void* stream);
+
 /* Fused flash-style attention on wgmma for wide heads (fp16, 160 < d <= 512, d % 8 == 0): the VAE decoder's single-head d = 512
  * self-attention, the AttentionFusedOps branch (src/onnxstream.cpp:6696-6929) without its [Tq, Tk] score buffer.  q [h,T,d], k [h,d,Tk]
  * when k_transposed (Tk % 8 == 0) else [h,Tk,d], v [h,Tk,d], out [h,T,d]; contiguous, 16-byte aligned.  No scratch: memory is the

@@ -17,6 +17,7 @@
 // sdpa_flash_kernel (below): the unpipelined structure for ScaledDotProductAttention with grouped KV heads and an additive mask --
 // llm.cpp's prompt prefill -- for d <= 128.
 // flash_attention_wide_kernel (below): 160 < d <= 512 -- the VAE decoder's single-head d = 512 attention -- with O split over its columns.
+// flash_attention_f32x_kernel (below): fp32 q / k / v / out on bf16 wgmma through the triple split, d <= 160.
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -841,6 +842,318 @@ int wd_launch(const void* q, const void* k, const void* v, const FaParams& p, in
     return launched(1);
 }
 
+// ---- fp32 multi-head attention on the tensor cores: bf16 triple split --------------------------------------------------------------
+// softmax(Q K^T * scale) V of flash_attention_kernel for fp32 q / k / v / out, to fp32 accuracy on bf16 wgmma.  Every operand is split
+// x = h + m + l into three bf16 planes (common.cuh: bf16x3_split) and every product into the six cross terms hh + hm + mh + hl + lh + mm
+// (the dropped ml, lm, ll are below ~2^-26 relative), all accumulated in fp32:
+//   f32x_split_kernel splits q, k and v (one launch for the three) into plane buffers [rows][3][heads*d], which the attention kernel reads
+//   through the strided tensor maps of the fp16 kernel: row stride 3 C, plane p of head h is "head" p * heads + h;
+//   S = Q K^T is 6 QKS wgmmas per key tile; the online softmax is f32x_softmax (fp32, expf, exact running maximum); P is split into
+//   three bf16 planes in registers and P V is 6 BK / 16 wgmmas per 64-column chunk of O, A from registers, V MN-major, added to O in fp32.
+// Roles as in sdpa_flash_kernel, unpipelined like it: one TMA producer warp (40 registers), two consumer warpgroups of 64 query rows
+// (232 registers), a K / V ring of KS stages.  Three planes take 3x the shared memory of the fp16 tiles:
+//   d <= 64:  64-key tiles, 2 stages: Q 48 KB + 2 x 48 KB;   registers O 32 + S 32 + P 3 x 16 + a P V chunk 32
+//   d <= 128: 32-key tiles, 2 stages: Q 96 KB + 2 x 48 KB;   O 64 + S 16 + P 3 x 8 + 32
+//   d <= 160: 32-key tiles, 1 stage:  Q 144 KB + 72 KB;      O 96 + S 16 + P 3 x 8 + 32
+template <int NCH, int BK, int QKS, int KS>
+struct F32xCfg {
+    static_assert(QKS <= 4 * NCH && (BK == 32 || BK == 64), "tile");
+    static constexpr int Q_CHUNK = BQ * 128;            // 128 rows x 64 bf16 columns
+    static constexpr int Q_PLANE = NCH * Q_CHUNK;
+    static constexpr int Q_BYTES = 3 * Q_PLANE;
+    static constexpr int KV_CHUNK = BK * 128;
+    static constexpr int KV_PLANE = NCH * KV_CHUNK;
+    static constexpr int KV_BYTES = 3 * KV_PLANE;       // one K (or V) tile: three planes
+    static constexpr int SMEM = Q_BYTES + KS * 2 * KV_BYTES + 1024 + 256;
+};
+
+// cross product x = 0..5 (hh, hm, mh, hl, lh, mm): plane of the A operand (Q, P) and of the B operand (K, V); 0 = h, 1 = m, 2 = l
+__host__ __device__ constexpr int x3a(int x) { return x == 2 || x == 5 ? 1 : (x == 4 ? 2 : 0); }
+__host__ __device__ constexpr int x3b(int x) { return x == 1 || x == 5 ? 1 : (x == 3 ? 2 : 0); }
+
+__device__ __forceinline__ uint32_t pack_bf162(__nv_bfloat16 lo, __nv_bfloat16 hi)
+{
+    __nv_bfloat162 b2 = __halves2bfloat162(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&b2);
+}
+
+// q [T, ldq], k / v [Tk, ldk / ldv] fp32 -> bf16 planes pq [T][3][C], pk / pv [Tk][3][C]; 4 columns per thread
+__global__ void f32x_split_kernel(const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, int64_t ldk, const float* __restrict__ v,
+                                  int64_t ldv, __nv_bfloat16* __restrict__ pq, __nv_bfloat16* __restrict__ pk, __nv_bfloat16* __restrict__ pv,
+                                  int64_t T, int64_t Tk, int C)
+{
+    osb_pdl_prologue();
+    const int C4 = C / 4;
+    const int64_t nq = T * C4, nk = Tk * C4, n = nq + 2 * nk;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const float* src = q; int64_t ld = ldq; __nv_bfloat16* dst = pq; int64_t e = i;
+        if (e >= nq) {
+            e -= nq;
+            if (e < nk) { src = k; ld = ldk; dst = pk; }
+            else { e -= nk; src = v; ld = ldv; dst = pv; }
+        }
+        const int64_t r = e / C4;
+        const int c = (int)(e - r * C4) * 4;
+        const float4 x = *reinterpret_cast<const float4*>(src + r * ld + c);
+        const float xs[4] = { x.x, x.y, x.z, x.w };
+        Vec<__nv_bfloat16, 4> h, m, l;
+#pragma unroll
+        for (int t = 0; t < 4; t++) bf16x3_split(xs[t], h.v[t], m.v[t], l.v[t]);
+        __nv_bfloat16* o = dst + r * 3 * C + c;
+        store_vec(o, h);
+        store_vec(o + C, m);
+        store_vec(o + 2 * C, l);
+    }
+}
+
+// Online softmax of one score tile for the fp32 kernel: fa_softmax with fp32 arithmetic -- the logit s * scale rounded once, as fp32
+// attention rounds it, and expf instead of the one-MUFU ex2 (whose ~2^-22 relative error and the rounding of scale * log2e show at fp32
+// accuracy); the exact running maximum.  Padding keys (last tile only) get -inf.
+template <int BK>
+__device__ __forceinline__ void f32x_softmax(float (&s)[BK / 2], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2], int key0, int cq, int Tk, float scale)
+{
+#pragma unroll
+    for (int c = 0; c < BK / 8; c++)
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+            const bool pad = key0 + 8 * c + cq + e >= Tk;
+            s[4 * c + e] = pad ? -INFINITY : s[4 * c + e] * scale;
+            s[4 * c + 2 + e] = pad ? -INFINITY : s[4 * c + 2 + e] * scale;
+        }
+    float m_new[2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float mt = -INFINITY;
+#pragma unroll
+        for (int c = 0; c < BK / 8; c++) mt = fmaxf(mt, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
+        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+        m_new[h] = fmaxf(m_run[h], mt);
+        alpha[h] = expf(m_run[h] - m_new[h]);                        // 0 on the first tile (m_run = -inf)
+        m_run[h] = m_new[h];
+    }
+    float lsum[2] = { 0.f, 0.f };
+#pragma unroll
+    for (int c = 0; c < BK / 8; c++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const float pe = expf(s[4 * c + 2 * h + e] - m_new[h]);
+                s[4 * c + 2 * h + e] = pe;
+                lsum[h] += pe;
+            }
+#pragma unroll
+    for (int h = 0; h < 2; h++) l_run[h] = l_run[h] * alpha[h] + lsum[h];
+}
+
+template <int BK>
+__device__ __forceinline__ void qk_mma_bf16(float (&s)[BK / 2], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    if constexpr (BK == 64) wgmma_m64n64k16_bf16<0>(s, da, db, scale_d);
+    else wgmma_m64n32k16_bf16<0>(s, da, db, scale_d);
+}
+
+template <int NCH, int BK, int QKS, int KS>
+__global__ void __launch_bounds__(FA_THREADS, 1)
+flash_attention_f32x_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+                            const FaParams p, float scale, float* __restrict__ out)
+{
+    using C = F32xCfg<NCH, BK, QKS, KS>;
+    osb_pdl_trigger_entry();
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint8_t* sQ = smem;
+    uint8_t* sK = sQ + C::Q_BYTES;
+    uint8_t* sV = sK + KS * C::KV_BYTES;
+    uint64_t* bars = (uint64_t*)(sV + KS * C::KV_BYTES);
+    uint64_t* q_full = bars;                           // [1]
+    uint64_t* kv_full = bars + 1;                      // [KS]
+    uint64_t* kv_empty = kv_full + KS;                 // [KS]: one arrival per consumer warp
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int head = blockIdx.y, heads = gridDim.y;
+    const int q0 = blockIdx.x * BQ;
+
+    if (warp == 0 && lane == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
+    }
+    if (warp == 1 && lane == 0) {
+        mbar_init(q_full, 1);
+        for (int i = 0; i < KS; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], FA_CONSUMERS / 32); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    osb_pdl_wait();
+
+    const int n_kv = p.kv_tiles;
+
+    if (warp < 4) {
+        setmaxnreg_dec<FA_PRODUCER_REGS>();
+        if (warp == 0) {
+            if (elect_one()) {
+                mbar_expect_tx(q_full, C::Q_BYTES);
+#pragma unroll
+                for (int pl = 0; pl < 3; pl++)
+#pragma unroll
+                    for (int c = 0; c < NCH; c++) tma_load_3d(sQ + pl * C::Q_PLANE + c * C::Q_CHUNK, &map_q, q_full, 64 * c, pl * heads + head, q0);
+            }
+            __syncwarp();
+            for (int j = 0; j < n_kv; j++) {
+                const int st = j % KS;
+                mbar_wait(&kv_empty[st], ((j / KS) & 1) ^ 1);
+                if (elect_one()) {
+                    mbar_expect_tx(&kv_full[st], 2 * C::KV_BYTES);
+#pragma unroll
+                    for (int pl = 0; pl < 3; pl++)
+#pragma unroll
+                        for (int c = 0; c < NCH; c++) {
+                            const int off = st * C::KV_BYTES + pl * C::KV_PLANE + c * C::KV_CHUNK;
+                            tma_load_3d(sK + off, &map_k, &kv_full[st], 64 * c, pl * heads + head, j * BK);
+                            tma_load_3d(sV + off, &map_v, &kv_full[st], 64 * c, pl * heads + head, j * BK);
+                        }
+                }
+                __syncwarp();
+            }
+        }
+    } else {
+        // ===================== warpgroups 1, 2: 64 query rows each =====================
+        setmaxnreg_inc<FA_CONSUMER_REGS>();
+        const int wg = (warp >> 2) - 1;
+        const int r = (warp & 3) * 16 + (lane >> 2);
+        const int cq = 2 * (lane & 3);
+        // Q / K K-major (32 B per 16-element k-step inside a 64-column chunk), V MN-major (16 keys = 2048 B per k-step); 8-row groups 1024 B apart
+        const uint64_t qdesc = make_smem_desc(smem_u32(sQ) + wg * (BQ / 2) * 128, 16, 1024);
+        const uint64_t kdesc0 = make_smem_desc(smem_u32(sK), 16, 1024);
+        const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), C::KV_CHUNK, 1024);
+        float o[NCH][32];
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+            for (int i = 0; i < 32; i++) o[ch][i] = 0.f;
+        float m_run[2] = { -INFINITY, -INFINITY }, l_run[2] = { 0.f, 0.f }, alpha[2];
+        mbar_wait(q_full, 0);
+        for (int j = 0; j < n_kv; j++) {
+            const int st = j % KS;
+            mbar_wait(&kv_full[st], (j / KS) & 1);
+            // S = sum of the six cross products over the k-steps.  The tensor cores' fp32 accumulation is not round-to-nearest: the five
+            // small products go first, while S is still small, and hh last.  The first MMA overwrites S.
+            const uint64_t kdesc = kdesc0 + (uint64_t)(st * C::KV_BYTES >> 4), vdesc = vdesc0 + (uint64_t)(st * C::KV_BYTES >> 4);
+            float s[BK / 2];
+            fence_regs(s);
+            wgmma_fence();
+#pragma unroll
+            for (int xx = 0; xx < 6; xx++)
+#pragma unroll
+                for (int k = 0; k < QKS; k++) {
+                    const int x = 5 - xx;
+                    qk_mma_bf16<BK>(s, qdesc + (uint64_t)(((x3a(x) * C::Q_PLANE + (k >> 2) * C::Q_CHUNK) >> 4) + (k & 3) * 2),
+                                    kdesc + (uint64_t)(((x3b(x) * C::KV_PLANE + (k >> 2) * C::KV_CHUNK) >> 4) + (k & 3) * 2), (k | xx) != 0);
+                }
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(s);
+            f32x_softmax<BK>(s, m_run, l_run, alpha, j * BK, cq, p.Tk, scale);
+            // O *= alpha; P (fp32 in s) -> three bf16 planes in the A-fragment order of the PV MMA (see fa_rescale_pack)
+#pragma unroll
+            for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+                for (int c = 0; c < 8; c++)
+#pragma unroll
+                    for (int h = 0; h < 2; h++) { o[ch][4 * c + 2 * h] *= alpha[h]; o[ch][4 * c + 2 * h + 1] *= alpha[h]; }
+            uint32_t a[3][BK / 16][4];
+#pragma unroll
+            for (int c = 0; c < BK / 8; c++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    __nv_bfloat16 p0[3], p1[3];
+                    bf16x3_split(s[4 * c + 2 * h], p0[0], p0[1], p0[2]);
+                    bf16x3_split(s[4 * c + 2 * h + 1], p1[0], p1[1], p1[2]);
+#pragma unroll
+                    for (int pl = 0; pl < 3; pl++) a[pl][c >> 1][(c & 1) * 2 + h] = pack_bf162(p0[pl], p1[pl]);
+                }
+            // O += P V one 64-column chunk at a time: the tile's product accumulates on the tensor cores in a fresh register tile (small
+            // products first, as for S) and is added to O in fp32 here, so O never takes a tensor-core accumulation over the whole sequence
+#pragma unroll
+            for (int pl = 0; pl < 3; pl++) fence_regs(a[pl]);
+#pragma unroll
+            for (int ch = 0; ch < NCH; ch++) {
+                float t[32];
+                fence_regs(t);
+                wgmma_fence();
+#pragma unroll
+                for (int xx = 0; xx < 6; xx++)
+#pragma unroll
+                    for (int kk = 0; kk < BK / 16; kk++) {
+                        const int x = 5 - xx;
+                        wgmma_m64n64k16_bf16_rs(t, a[x3a(x)][kk], vdesc + (uint64_t)((x3b(x) * C::KV_PLANE + ch * C::KV_CHUNK + kk * 2048) >> 4), (kk | xx) != 0);
+                    }
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(t);
+#pragma unroll
+                for (int i = 0; i < 32; i++) o[ch][i] += t[i];
+            }
+#pragma unroll
+            for (int pl = 0; pl < 3; pl++) fence_regs(a[pl]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&kv_empty[st]);
+        }
+        // epilogue: O / l -> out[q, head*d + c] (fp32)
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            float l = l_run[h];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = 1.f / l;
+            const int qrow = q0 + wg * (BQ / 2) + r + 8 * h;
+            if (qrow >= p.T) continue;
+            float* orow = out + (long long)qrow * p.ldo + (long long)head * p.d;
+#pragma unroll
+            for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+                for (int c = 0; c < 8; c++) {
+                    const int col = 64 * ch + 8 * c + cq;
+                    if (col < p.d)     // d % 8 == 0: the pair is inside
+                        *reinterpret_cast<float2*>(orow + col) = make_float2(o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
+                }
+        }
+    }
+}
+
+// Every tensor map is made before anything is enqueued, so a refused launch enqueues nothing.  The plane buffers hold 2-byte elements
+// that the tensor maps only move: head_map's fp16 element type serves for bf16.
+template <int NCH, int BK, int QKS, int KS>
+int f32x_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, float* out, FaParams p, float scale,
+                int64_t heads, __nv_bfloat16* planes, cudaStream_t st)
+{
+    using Cf = F32xCfg<NCH, BK, QKS, KS>;
+    const int64_t C = heads * p.d;
+    __nv_bfloat16* pq = planes;
+    __nv_bfloat16* pk = pq + 3 * p.T * C;
+    __nv_bfloat16* pv = pk + 3 * p.Tk * C;
+    CUtensorMap mq, mk, mv;
+    if (!head_map(&mq, pq, p.d, (int)(3 * heads), p.T, 3 * C, BQ) || !head_map(&mk, pk, p.d, (int)(3 * heads), p.Tk, 3 * C, BK) ||
+        !head_map(&mv, pv, p.d, (int)(3 * heads), p.Tk, 3 * C, BK))
+        return (int)cudaErrorInvalidValue;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(flash_attention_f32x_kernel<NCH, BK, QKS, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cf::SMEM);
+        if (e != cudaSuccess) return (int)e;
+        attr = true;
+    }
+    osb_launch((f32x_split_kernel), grid_for((size_t)((p.T + 2 * (int64_t)p.Tk) * C / 4), 256), 256, 0, st, q, ldq, k, ldk, v, ldv, pq, pk, pv,
+               (int64_t)p.T, (int64_t)p.Tk, (int)C);
+    const int e = launched();
+    if (e) return e;
+    p.kv_tiles = (p.Tk + BK - 1) / BK;
+    dim3 grid((unsigned)((p.T + BQ - 1) / BQ), (unsigned)heads);
+    osb_launch((flash_attention_f32x_kernel<NCH, BK, QKS, KS>), grid, FA_THREADS, (size_t)Cf::SMEM, st, mq, mk, mv, p, scale, out);
+    return launched(1);
+}
+
 }  // namespace
 
 extern "C" int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
@@ -867,6 +1180,35 @@ extern "C" int osb_flash_attention(const void* q, int64_t ldq, const void* k, in
     if (d <= 80) return fa_launch<2, 64, 5>(q, ldq, k, ldk, v, ldv, p, heads, st);
     if (d <= 128) return fa_launch<2, 64, 8>(q, ldq, k, ldk, v, ldv, p, heads, st);
     return fa_launch<3, 32, 10>(q, ldq, k, ldk, v, ldv, p, heads, st);
+}
+
+extern "C" int osb_flash_attention_f32x_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
+{
+    return dtype == OSB_F32 && d >= 8 && d <= 160 && d % 8 == 0 && T >= 1 && Tk >= 1 && T <= (int64_t)INT32_MAX - BQ && Tk <= (int64_t)INT32_MAX - BKV &&
+           fa_encode() != nullptr;
+}
+
+// osb_flash_attention for fp32 q / k / v / out (row strides in floats, multiples of 4, >= heads * d; 16-byte aligned pointers), planes: scratch
+// of 6 (T + 2 Tk) heads d bytes for the bf16 planes.  Two launches: the split, then the attention.
+extern "C" int osb_flash_attention_f32x(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
+                                        int64_t heads, int64_t T, int64_t Tk, int64_t d, float scale, void* planes, void* stream)
+{
+    if (!osb_flash_attention_f32x_ok(T, Tk, d, OSB_F32) || heads < 1 || heads > 65535 || !(scale > 0.f) || !(scale < INFINITY)) return (int)cudaErrorInvalidValue;
+    const int64_t C = heads * d;
+    if (ldq < C || ldk < C || ldv < C || ldo < C || (ldq % 4) || (ldk % 4) || (ldv % 4) || (ldo % 4) || C > INT32_MAX) return (int)cudaErrorInvalidValue;
+    if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out | (uintptr_t)planes) & 15) != 0) return (int)cudaErrorInvalidValue;
+    FaParams p{};
+    p.T = (int)T; p.Tk = (int)Tk; p.d = (int)d;
+    p.out = nullptr; p.ldo = ldo;
+    const float* fq = (const float*)q; const float* fk = (const float*)k; const float* fv = (const float*)v;
+    float* fo = (float*)out;
+    __nv_bfloat16* pl = (__nv_bfloat16*)planes;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (d <= 48) return f32x_launch<1, 64, 3, 2>(fq, ldq, fk, ldk, fv, ldv, fo, p, scale, heads, pl, st);
+    if (d <= 64) return f32x_launch<1, 64, 4, 2>(fq, ldq, fk, ldk, fv, ldv, fo, p, scale, heads, pl, st);
+    if (d <= 80) return f32x_launch<2, 32, 5, 2>(fq, ldq, fk, ldk, fv, ldv, fo, p, scale, heads, pl, st);
+    if (d <= 128) return f32x_launch<2, 32, 8, 2>(fq, ldq, fk, ldk, fv, ldv, fo, p, scale, heads, pl, st);
+    return f32x_launch<3, 32, 10, 1>(fq, ldq, fk, ldk, fv, ldv, fo, p, scale, heads, pl, st);
 }
 
 extern "C" int osb_flash_attention_wide_ok(int64_t T, int64_t Tk, int64_t d, int dtype)

@@ -3,6 +3,7 @@
 
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include <algorithm>
 #include <utility>
@@ -104,6 +105,16 @@ __device__ __forceinline__ float to_float(uint8_t v) { return (float)v; }
 template <typename T> __device__ __forceinline__ T from_float(float v);
 template <> __device__ __forceinline__ float from_float<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half from_float<__half>(float v) { return __float2half_rn(v); }
+
+// ---- fp32 -> bf16 triple split of the tensor-core fp32 paths (osb_tc_gemm_f32x, osb_flash_attention_f32x) ----------------------------
+// x = h + m + l, h = bf16(x), m = bf16(x - h), l = bf16(x - h - m): 24 mantissa bits in three bf16 planes
+__device__ __forceinline__ void bf16x3_split(float x, __nv_bfloat16& h, __nv_bfloat16& m, __nv_bfloat16& l)
+{
+    h = __float2bfloat16_rn(x);
+    const float r1 = x - __bfloat162float(h);
+    m = __float2bfloat16_rn(r1);
+    l = __float2bfloat16_rn(r1 - __bfloat162float(m));
+}
 
 // ---- 128-bit vectors -------------------------------------------------------------------------------------------
 template <typename T, int N> struct alignas(sizeof(T) * N) Vec { T v[N]; };

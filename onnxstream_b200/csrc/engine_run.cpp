@@ -91,6 +91,14 @@ struct Engine::Impl {
     std::map<size_t, MhaKV> mha_kv;                    // step -> K / V projections computed ahead on the side stream (valid for one run)
     void mha_project(size_t i, const Tensor& x, const Tensor* xq, Tensor* ql, Tensor& kl, Tensor& vl, int64_t Tka);
     void mha_prepass(size_t si);
+    // fused flash kernel (K / V projections of exactly Tk rows) or the GEMM -> softmax -> GEMM chain (Tk padded to 8): one rule for
+    // mha_prepass and fused_mha, which must agree on the K / V buffers
+    bool mha_flash(int64_t T, int64_t Tk, int64_t d, DType ty, float scale) const
+    {
+        if (!E.flash_attention || E.gemm_impl == 1) return false;
+        if (ty == DType::f32) return scale > 0.f && osb_flash_attention_f32x_ok(T, Tk, d, K(ty));
+        return osb_flash_attention_ok(T, Tk, d, K(ty));
+    }
 
     // int64 graph inputs and CUDA graphs: an op that consumes the host VALUES of such a tensor (other than through its device mirror)
     // makes the run un-capturable -- a replay would reuse the values of the captured run
@@ -1845,7 +1853,8 @@ void Engine::Impl::mha_prepass(size_t si)
     if (xk.type != DType::f16 && xk.type != DType::f32) return;
     auto& qs = E.m_ops[i + 3].out[0].shape; auto& kts = E.m_ops[i + 8].out[0].shape;
     const int64_t h = qs[0], T = qs[1], d = qs[2], Tk = kts[2], C = h * d;
-    const bool use_flash = E.flash_attention && E.gemm_impl != 1 && osb_flash_attention_ok(T, Tk, d, K(ty));
+    const float scale = ty == DType::f32 ? scalar_of(in(i + 14, 1), E.m_ops[i + 14]) : 1.f;     // only the fp32 kernel's rule reads it
+    const bool use_flash = mha_flash(T, Tk, d, ty, scale);
     const int64_t Tka = use_flash ? Tk : ((Tk + 7) & ~(int64_t)7);
     Tensor proxy; proxy.type = ty;      // only the dtype of the query side matters here
     MhaKV kv;
@@ -1877,7 +1886,7 @@ void Engine::Impl::fused_mha(const Step& s)
     if (ty == DType::f16) scale = __half2float(__float2half_rn(scale));
     if (x.shape[2] != wq.shape[0] || xk.shape[2] != wk.shape[0] || xv.shape[2] != wv.shape[0]) throw std::runtime_error("XnnPack::matrix_multiply_fp32: invalid shape of inputs.");
 
-    const bool use_flash = E.flash_attention && E.gemm_impl != 1 && osb_flash_attention_ok(T, Tk, d, K(ty));
+    const bool use_flash = mha_flash(T, Tk, d, ty, scale);
     // the flash kernel reads K / V through tensor maps of exactly Tk rows (rows beyond are zero-filled by TMA): no padding needed
     const int64_t Tka = use_flash ? Tk : Tkp;
     Tensor ql = make(ty, { T, C }), kl, vl, out = make(ty, { 1, T, C });
@@ -1895,7 +1904,13 @@ void Engine::Impl::fused_mha(const Step& s)
 
     if (use_flash) {
         // one kernel: QK^T -> online softmax -> PV with the score tile in registers
-        ck(osb_flash_attention(ql.data(), C, kl.data(), C, vl.data(), C, out.mdata(), C, h, T, Tk, d, scale, st), "osb_flash_attention");
+        if (ty == DType::f32) {
+            // fp32: the launch first splits q, k, v into bf16 planes (6 bytes per element) in this scratch
+            Tensor planes = make(DType::f16, { 3 * (T + 2 * Tk) * C });
+            ck(osb_flash_attention_f32x(ql.data(), C, kl.data(), C, vl.data(), C, out.mdata(), C, h, T, Tk, d, scale, planes.mdata(), st), "osb_flash_attention_f32x");
+        } else {
+            ck(osb_flash_attention(ql.data(), C, kl.data(), C, vl.data(), C, out.mdata(), C, h, T, Tk, d, scale, st), "osb_flash_attention");
+        }
         push(i + 19, 0, out);
         return;
     }

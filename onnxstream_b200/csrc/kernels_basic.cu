@@ -1123,14 +1123,12 @@ int osb_binary(int op, const void* a, const int64_t* as, const void* b, const in
 }
 
 // ---- fp32 -> bf16 triple split, expanded along K for the tensor-core fp32 path (gemm_wgmma.cu: osb_tc_gemm_f32x) -----------------
-// x = h + m + l, h = bf16(x), m = bf16(x - h), l = bf16(x - h - m).  A side: segments [h|h|m|h|l|m]; B side: [h|m|h|l|h|m], so that
-// segment s of A times segment s of B runs over the six products hh, hm, mh, hl, lh, mm.
+// x = h + m + l (common.cuh: bf16x3_split).  A side: segments [h|h|m|h|l|m]; B side: [h|m|h|l|h|m], so that segment s of A times
+// segment s of B runs over the six products hh, hm, mh, hl, lh, mm.
 __device__ __forceinline__ void bf16x3_parts(float x, int b_side, __nv_bfloat16* six)
 {
-    const __nv_bfloat16 h = __float2bfloat16_rn(x);
-    const float r1 = x - __bfloat162float(h);
-    const __nv_bfloat16 m = __float2bfloat16_rn(r1);
-    const __nv_bfloat16 l = __float2bfloat16_rn(r1 - __bfloat162float(m));
+    __nv_bfloat16 h, m, l;
+    bf16x3_split(x, h, m, l);
     if (b_side) { six[0] = h; six[1] = m; six[2] = h; six[3] = l; six[4] = h; six[5] = m; }
     else        { six[0] = h; six[1] = h; six[2] = m; six[3] = h; six[4] = l; six[5] = m; }
 }

@@ -24,6 +24,13 @@ Prints ONE JSON line: the card (name, power limit, max SM clock, read with an nv
   trace : (--trace DIR) per-kernel-name GPU time of one eager SD 1.5 UNet step (64x64 latent, fp16, resident weights, no CUDA graph)
           and the attention share: flash_attention_kernel, softmax_scaled_* and the tensor-core GEMM launched right before and right
           after each softmax (the QK^T / PV pair) over all kernel and memset time.  The chrome trace is written to DIR.
+  f32   : (--f32) the fp32 attentions instead of the fp16 ones: the SD 1.5 shapes above and SDXL's d = 64 (10 heads at 64^2 with the
+          77-token context, 20 heads at 32^2), ms per call for
+            flash  : osb_flash_attention_f32x (bf16 triple split; the plane split launch included)
+            chain  : the fp32 chain: osb_gemm_ld(QK^T) -> osb_softmax_scaled_ld -> osb_gemm_ld(PV) on the CUDA cores through an fp32
+                     [h, T, Tk padded to 8] score buffer
+          TFLOP/s of algorithmic fp32 work (4*h*T*Tk*d / t), the score buffer the chain allocates, max|flash - chain|.  With --trace
+          the traced step is the fp32 UNet (fp32 weights and arithmetic).
 OSB_ENGINE_LIB selects the engine library (build variants).  Needs a CUDA device; everything else it writes goes to a temporary
 directory.
 """
@@ -41,7 +48,7 @@ sys.path.insert(0, ROOT)
 from onnxstream_b200 import emit  # noqa: E402
 from onnxstream_b200.model import ENGINE_LIB, Model  # noqa: E402
 
-F16 = 2
+F16, F32 = 2, 3
 HEADS = 8
 SHAPES = [
     # name, T, Tk, d
@@ -119,6 +126,63 @@ def kernel_level(iters, warmup, clock_hz):
                         "max_abs_diff": float((o_flash.float() - o_chain.float()).abs().max())})
         out.append(row)
         del q, k, v, S, o_flash, o_chain
+        torch.cuda.empty_cache()
+    return out
+
+
+# (name, heads, T, Tk, d): the SD 1.5 levels (8 heads) and SDXL's d = 64 levels
+F32_SHAPES = [(n, HEADS, T, Tk, d) for n, T, Tk, d in SHAPES] + [("xl_64sq_cross", 10, 4096, 77, 64), ("xl_32sq_self", 20, 1024, 1024, 64)]
+
+
+def kernel_level_f32(iters, warmup):
+    import torch
+    lib = ctypes.CDLL(ENGINE_LIB)
+    vp, i64, cf, ci = ctypes.c_void_p, ctypes.c_int64, ctypes.c_float, ctypes.c_int
+    lib.osb_flash_attention_f32x.argtypes = [vp, i64, vp, i64, vp, i64, vp, i64, i64, i64, i64, i64, cf, vp, vp]
+    lib.osb_gemm_ld.argtypes = [vp, i64, vp, i64, vp, i64, vp, vp, i64, i64, i64, i64, i64, i64, i64, ci, ci, ci, vp]
+    lib.osb_softmax_scaled_ld.argtypes = [vp, vp, ci, i64, i64, i64, cf, vp, i64, vp]
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    out = []
+    for name, h, T, Tk, d in F32_SHAPES:
+        C = h * d
+        Tkp = (Tk + 7) // 8 * 8
+        g = torch.Generator(device="cuda").manual_seed(T * 7 + Tk + d)
+        q = torch.randn(T, C, device="cuda", generator=g)
+        k = torch.zeros(Tkp, C, device="cuda"); k[:Tk] = torch.randn(Tk, C, device="cuda", generator=g)
+        v = torch.zeros(Tkp, C, device="cuda"); v[:Tk] = torch.randn(Tk, C, device="cuda", generator=g)
+        S = torch.empty(h, T, Tkp, device="cuda")
+        planes = torch.empty(3 * (T + 2 * Tk) * C, device="cuda", dtype=torch.bfloat16)
+        o_flash = torch.zeros(T, C, device="cuda")
+        o_chain = torch.zeros(T, C, device="cuda")
+        scale = 1.0 / d ** 0.5
+
+        def flash():
+            assert lib.osb_flash_attention_f32x(q.data_ptr(), C, k.data_ptr(), C, v.data_ptr(), C, o_flash.data_ptr(), C, h, T, Tk, d, scale,
+                                                planes.data_ptr(), stream) == 0
+
+        def chain():
+            assert lib.osb_gemm_ld(q.data_ptr(), C, k.data_ptr(), C, S.data_ptr(), Tkp, None, None, h, T, Tkp, d, d, d, T * Tkp, 1, F32, 0, stream) == 0
+            assert lib.osb_softmax_scaled_ld(S.data_ptr(), S.data_ptr(), F32, h * T, Tk, Tkp, scale, None, 1, stream) == 0
+            assert lib.osb_gemm_ld(S.data_ptr(), Tkp, v.data_ptr(), C, o_chain.data_ptr(), C, None, None, h, T, d, Tkp, T * Tkp, d, d, 0, F32, 0, stream) == 0
+
+        def timed(fn):
+            for _ in range(warmup):
+                fn()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(iters):
+                fn()
+            e1.record()
+            torch.cuda.synchronize()
+            return e0.elapsed_time(e1) / iters
+
+        t_flash, t_chain = timed(flash), timed(chain)
+        flop = 4.0 * h * T * Tk * d
+        out.append({"shape": name, "h": h, "T": T, "Tk": Tk, "d": d, "flash_ms": round(t_flash, 4), "chain_ms": round(t_chain, 4),
+                    "flash_tflops": round(flop / t_flash / 1e9, 2), "chain_tflops": round(flop / t_chain / 1e9, 2),
+                    "flash_vs_chain": round(t_chain / t_flash, 2), "score_buffer_mb": round(h * T * Tkp * 4 / 2 ** 20, 1),
+                    "max_abs_diff": float((o_flash - o_chain).abs().max())})
+        del q, k, v, S, planes, o_flash, o_chain
         torch.cuda.empty_cache()
     return out
 
@@ -210,17 +274,18 @@ def tiled_level(runs):
             "max_abs_diff": float(np.abs(imgs[1] - imgs[0]).max())}
 
 
-def trace_step(trace_dir):
-    """One eager SD 1.5 UNet step under torch.profiler (CUDA activities); per-kernel GPU time and attention's share of it."""
+def trace_step(trace_dir, f32=False):
+    """One eager SD 1.5 UNet step (fp16, or f32: fp32 weights and arithmetic) under torch.profiler (CUDA activities); per-kernel GPU time
+    and attention's share of it."""
     import torch
     from torch.profiler import ProfilerActivity, profile
     cfg = emit.UNetConfig.sd15(64)
     d = tempfile.mkdtemp(prefix="osb200_attn_trace_") + "/"
     try:
-        emit.emit_unet(d, cfg, "float16", seed=0)
+        emit.emit_unet(d, cfg, "float32" if f32 else "float16", seed=0)
         inputs = emit.unet_inputs(cfg)
         m = Model(ENGINE_LIB, 0, "ram+nocache")
-        for o in ("use_fp16_arithmetic", "fuse_ops_in_attention"):
+        for o in (() if f32 else ("use_fp16_arithmetic", "fuse_ops_in_attention")):
             m.set_option(o, True)
         m.lib.model_set_option(m.h, b"b200_resident_weights", 1)
         m.lib.model_set_option(m.h, b"b200_cuda_graph", 0)
@@ -251,7 +316,7 @@ def trace_step(trace_dir):
     attn = [False] * len(ev)
     for i, e in enumerate(ev):
         n = e["name"]
-        if "flash_attention_kernel" in n:
+        if "flash_attention_kernel" in n or "flash_attention_f32x_kernel" in n or "f32x_split_kernel" in n:
             attn[i] = True
         elif "softmax_scaled" in n:
             attn[i] = True
@@ -260,7 +325,7 @@ def trace_step(trace_dir):
             j = i - 1
             while j >= 0 and ev[j]["args"].get("stream") != s:
                 j -= 1
-            if j >= 0 and "tc_gemm" in ev[j]["name"]:
+            if j >= 0 and ("tc_gemm" in ev[j]["name"] or "igemm" in ev[j]["name"]):
                 attn[j] = True
                 j -= 1
                 while j >= 0 and (ev[j]["args"].get("stream") != s or ev[j]["cat"] == "gpu_memset"):
@@ -270,7 +335,7 @@ def trace_step(trace_dir):
             j = i + 1
             while j < len(ev) and ev[j]["args"].get("stream") != s:
                 j += 1
-            if j < len(ev) and "tc_gemm" in ev[j]["name"]:
+            if j < len(ev) and ("tc_gemm" in ev[j]["name"] or "igemm" in ev[j]["name"]):
                 attn[j] = True
     total = sum(e["dur"] for e in ev)
     attn_us = sum(e["dur"] for e, a in zip(ev, attn) if a)
@@ -294,6 +359,7 @@ def main():
     ap.add_argument("--trace", default=None, metavar="DIR", help="also trace one eager UNet step and write the chrome trace to DIR")
     ap.add_argument("--skip-kernels", action="store_true")
     ap.add_argument("--vae", action="store_true", help="time the VAE's d = 512 attention shapes instead of the UNet's")
+    ap.add_argument("--f32", action="store_true", help="time the fp32 attentions (and trace the fp32 UNet) instead of the fp16 ones")
     ap.add_argument("--tiled-runs", type=int, default=7, help="--vae: timed tiled decodes per setting (0 = skip)")
     a = ap.parse_args()
     import torch
@@ -305,10 +371,12 @@ def main():
         res["vae"] = vae_level(a.iters, a.warmup)
         if a.tiled_runs:
             res["tiled"] = tiled_level(a.tiled_runs)
+    elif a.f32 and not a.skip_kernels:
+        res["kernel"] = kernel_level_f32(a.iters, a.warmup)
     elif not a.skip_kernels:
         res["kernel"] = kernel_level(a.iters, a.warmup, float(c["max_sm_clock"].split()[0]) * 1e6)
     if a.trace:
-        res["trace"] = trace_step(a.trace)
+        res["trace"] = trace_step(a.trace, a.f32)
     print(json.dumps(res))
 
 
