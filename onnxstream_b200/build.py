@@ -22,7 +22,7 @@ CXX = os.environ.get("OSB_CXX", "/usr/bin/g++")
 
 CU_SOURCES = ["kernels_basic.cu", "kernels_gemm.cu", "gemm_wgmma.cu", "attention_wgmma.cu"]
 CPP_SOURCES = ["engine.cpp", "engine_run.cpp", "plan.cpp", "capi.cpp", "comm.cpp", "workspace.cpp"]
-HEADERS = ["common.cuh", "engine.h", "engine_impl.h", "plan.h", "workspace.h", "../../include/onnxstream_b200_kernels.h", "../../include/onnxstream_b200.h"]
+HEADERS = ["common.cuh", "tc_ptx.cuh", "gemm_i8.cuh", "engine.h", "engine_impl.h", "plan.h", "workspace.h", "../../include/onnxstream_b200_kernels.h", "../../include/onnxstream_b200.h"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
               "-Xcompiler", "-fPIC", "-ccbin", CXX] + os.environ.get("OSB_NVCC_EXTRA", "").split()

@@ -21,11 +21,8 @@
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
-#include <cstdlib>
 #include <cuda.h>
-#include <cudaTypedefs.h>
 #include <cstdio>
-#include <mutex>
 
 namespace {
 
@@ -42,24 +39,84 @@ constexpr int FA_PRODUCER_REGS = 40, FA_CONSUMER_REGS = 232;     // 128 * 40 + 2
 // zero-filled by TMA), BK = keys per tile, QKS = k-steps of 16 in Q K^T (ceil(d / 16) rounded to an instantiation).  Registers per
 // consumer thread: O 32 * NCH, S BK / 2, P BK / 4 -- d <= 64: 128-key tiles (32 + 64 + 32), d <= 128: 64-key tiles (64 + 32 + 16),
 // d <= 160: 32-key tiles (96 + 16 + 8; with 64-key tiles ptxas spills and serialises the wgmmas).
-template <int NCH, int BK, int QKS>
+// The same layout serves the other 128-query kernels: KS = stages of the K / V ring, PLANES = operand planes per tile (3: the bf16 triple
+// split of flash_attention_f32x_kernel).  Shared memory: Q, the K ring, the V ring, then the mbarriers at BARS.
+template <int NCH, int BK, int QKS, int KS = KV_STAGES, int PLANES = 1>
 struct FaCfg {
     static_assert(QKS <= 4 * NCH && (BK == 32 || BK == 64 || BK == 128), "tile");
-    static constexpr int Q_CHUNK = BQ * 128;            // 128 rows x 64 fp16 columns
+    static constexpr int Q_CHUNK = BQ * 128;            // 128 rows x 64 2-byte columns
     static constexpr int KV_CHUNK = BK * 128;
-    static constexpr int Q_BYTES = NCH * Q_CHUNK;
-    static constexpr int KV_BYTES = NCH * KV_CHUNK;     // one K (or V) tile
-    static constexpr int SMEM = Q_BYTES + KV_STAGES * 2 * KV_BYTES + 1024 + 256;
+    static constexpr int Q_PLANE = NCH * Q_CHUNK;
+    static constexpr int KV_PLANE = NCH * KV_CHUNK;
+    static constexpr int Q_BYTES = PLANES * Q_PLANE;
+    static constexpr int KV_BYTES = PLANES * KV_PLANE;  // one K (or V) tile
+    static constexpr int BARS = Q_BYTES + KS * 2 * KV_BYTES;
+    static constexpr int SMEM = BARS + 1024 + 256;
 };
 
 struct FaParams {
     int T, Tk, d;
     int kv_tiles;
     float scale_log2;        // scale * log2(e)
-    float tau;               // lazy-rescaling threshold in log2 units (0 = exact running maximum)
     __half* out;             // [T, ldo] merged layout, head h at column h*d
     long long ldo;
 };
+
+// Kernel entry of the flash kernels after the PDL trigger, up to the wait for the previous grid: the dynamic shared memory aligned to 1024 bytes (128B-swizzled
+// TMA boxes and wgmma operands), the three tensor maps prefetched and the mbarriers at smem + bar_off initialised -- q_full, then the
+// n0 full and n0 empty barriers of the first ring, then the n1 full and n1 empty barriers of the second.  Full barriers take the
+// producer's arrival (and the TMA bytes), empty barriers `arrivals` consumer arrivals.  Returns the aligned shared memory.
+__device__ __forceinline__ uint8_t* fa_prologue(const CUtensorMap* map_q, const CUtensorMap* map_k, const CUtensorMap* map_v, int bar_off,
+                                                uint32_t arrivals, int n0, int n1 = 0)
+{
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp == 0 && lane == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(map_q) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(map_k) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(map_v) : "memory");
+    }
+    if (warp == 1 && lane == 0) {
+        uint64_t* bars = (uint64_t*)(smem + bar_off);
+        mbar_init(bars, 1);
+        for (int i = 0; i < n0; i++) { mbar_init(&bars[1 + i], 1); mbar_init(&bars[1 + n0 + i], arrivals); }
+        for (int i = 0; i < n1; i++) { mbar_init(&bars[1 + 2 * n0 + i], 1); mbar_init(&bars[1 + 2 * n0 + n1 + i], arrivals); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    osb_pdl_wait();
+    return smem;
+}
+
+// Producer warp of a K / V ring of KS stages: for key tile j, wait until the consumers have released slot j % KS, expect its bytes and
+// issue its loads on one lane (load(slot, j, &kv_full[slot])).
+template <int KS, typename Load>
+__device__ __forceinline__ void fa_produce_kv(uint64_t* kv_full, uint64_t* kv_empty, int n_kv, uint32_t tile_bytes, Load load)
+{
+    for (int j = 0; j < n_kv; j++) {
+        const int st = j % KS;
+        mbar_wait(&kv_empty[st], ((j / KS) & 1) ^ 1);
+        if (elect_one()) {
+            mbar_expect_tx(&kv_full[st], tile_bytes);
+            load(st, j, &kv_full[st]);
+        }
+        __syncwarp();
+    }
+    osb_pdl_trigger_late();
+}
+
+// The maximum of score row r + 8h (s in the accumulator fragment, see fa_softmax): this thread's columns, then its quad's.
+template <int BK>
+__device__ __forceinline__ float fa_row_max(const float (&s)[BK / 2], int h)
+{
+    float mt = -INFINITY;
+#pragma unroll
+    for (int c = 0; c < BK / 8; c++) mt = fmaxf(mt, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
+    mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+    mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+    return mt;
+}
 
 // 2^x on the SFU, flush-to-zero: one MUFU.EX2 (exp2f() adds a range check and two scaling multiplies for denormal results,
 // which a probability that is about to be rounded to fp16 does not need).  ex2(-inf) = +0.
@@ -74,6 +131,31 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi)
 {
     __half2 h2 = __floats2half2_rn(lo, hi);
     return *reinterpret_cast<uint32_t*>(&h2);
+}
+
+__device__ __forceinline__ void store_pair(__half* p, float lo, float hi) { *reinterpret_cast<uint32_t*>(p) = pack_half2(lo, hi); }
+__device__ __forceinline__ void store_pair(float* p, float lo, float hi) { *reinterpret_cast<float2*>(p) = make_float2(lo, hi); }
+
+// Epilogue: O / l -> out.  The quad sums its partial row sums; rows[h] is this thread's output row r + 8h (nullptr past the last row),
+// which takes the column pairs 64 ch + 8 c + cq, + 1 below ncols (d % 8 == 0: a pair is inside or outside as a whole).
+template <typename OutT, int NCH>
+__device__ __forceinline__ void fa_store(const float (&o)[NCH][32], const float (&l_run)[2], OutT* const (&rows)[2], int ncols, int cq)
+{
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = 1.f / l;
+        if (!rows[h]) continue;
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+            for (int c = 0; c < 8; c++) {
+                const int col = 64 * ch + 8 * c + cq;
+                if (col < ncols) store_pair(rows[h] + col, o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
+            }
+    }
 }
 
 template <int BK>
@@ -132,15 +214,9 @@ __device__ __forceinline__ void fa_softmax(float (&s)[BK / 2], float (&m_run)[2]
     float neg_m[2];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-        float mt = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < BK / 8; c++) mt = fmaxf(mt, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
-        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
-        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
-        // Lazy rescaling: the stale maximum is kept while the new one exceeds it by at most tau (log2 units) -- P <= 2^tau stays well
-        // inside fp16, O and l accumulate in fp32.  tau = 0 is the exact running maximum (the default; OSB_FLASH_TAU sets it).
-        const float m_cand = fmaxf(m_run[h], mt * p.scale_log2);     // scale_log2 > 0
-        const float m_new = (m_cand - m_run[h] > p.tau) ? m_cand : m_run[h];
+        // the maximum of the raw scores times scale_log2 is the maximum of the scaled logits only for scale > 0: the entries refuse
+        // other scales
+        const float m_new = fmaxf(m_run[h], fa_row_max<BK>(s, h) * p.scale_log2);
         alpha[h] = ex2_approx(m_run[h] - m_new);                     // 0 on the first tile (m_run = -inf)
         neg_m[h] = -m_new;
         m_run[h] = m_new;
@@ -186,34 +262,17 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_c
     using C = FaCfg<NCH, BK, QKS>;
     constexpr int S = KV_STAGES;
     osb_pdl_trigger_entry();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t* sQ = smem;
-    uint8_t* sK = sQ + C::Q_BYTES;
-    uint8_t* sV = sK + S * C::KV_BYTES;
-    uint64_t* bars = (uint64_t*)(sV + S * C::KV_BYTES);
-    uint64_t* q_full = bars;                           // [1]
-    uint64_t* kv_full = bars + 1;                      // [S]
-    uint64_t* kv_empty = kv_full + S;                  // [S]: one arrival per consumer warp
-
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int head = blockIdx.y;
     const int q0 = blockIdx.x * BQ;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        mbar_init(q_full, 1);
-        for (int i = 0; i < S; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], FA_CONSUMERS / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    osb_pdl_wait();
-
     const int n_kv = p.kv_tiles;
+    uint8_t* smem = fa_prologue(&map_q, &map_k, &map_v, C::BARS, FA_CONSUMERS / 32, S);   // kv_empty: one arrival per consumer warp
+    uint8_t* sQ = smem;
+    uint8_t* sK = sQ + C::Q_BYTES;
+    uint8_t* sV = sK + S * C::KV_BYTES;
+    uint64_t* q_full = (uint64_t*)(smem + C::BARS);   // [1]
+    uint64_t* kv_full = q_full + 1;                    // [S]
+    uint64_t* kv_empty = kv_full + S;                  // [S]
 
     if (warp < 4) {
         setmaxnreg_dec<FA_PRODUCER_REGS>();
@@ -224,19 +283,13 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_c
                 for (int c = 0; c < NCH; c++) tma_load_3d(sQ + c * C::Q_CHUNK, &map_q, q_full, 64 * c, head, q0);
             }
             __syncwarp();
-            for (int j = 0; j < n_kv; j++) {
-                const int st = j % S;
-                mbar_wait(&kv_empty[st], ((j / S) & 1) ^ 1);
-                if (elect_one()) {
-                    mbar_expect_tx(&kv_full[st], 2 * C::KV_BYTES);
+            fa_produce_kv<S>(kv_full, kv_empty, n_kv, 2 * C::KV_BYTES, [&](int st, int j, uint64_t* bar) {
 #pragma unroll
-                    for (int c = 0; c < NCH; c++) {
-                        tma_load_3d(sK + st * C::KV_BYTES + c * C::KV_CHUNK, &map_k, &kv_full[st], 64 * c, head, j * BK);
-                        tma_load_3d(sV + st * C::KV_BYTES + c * C::KV_CHUNK, &map_v, &kv_full[st], 64 * c, head, j * BK);
-                    }
+                for (int c = 0; c < NCH; c++) {
+                    tma_load_3d(sK + st * C::KV_BYTES + c * C::KV_CHUNK, &map_k, bar, 64 * c, head, j * BK);
+                    tma_load_3d(sV + st * C::KV_BYTES + c * C::KV_CHUNK, &map_v, bar, 64 * c, head, j * BK);
                 }
-                __syncwarp();
-            }
+            });
         }
     } else {
         // ===================== warpgroups 1, 2: 64 query rows each =====================
@@ -297,52 +350,29 @@ flash_attention_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_c
         wgmma_wait<0>();
 #pragma unroll
         for (int ch = 0; ch < NCH; ch++) fence_regs(o[ch]);
-        // epilogue: O / l -> fp16 -> out[q, head*d + c]
+        // out[q, head*d + c]
+        __half* rows[2];
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-            float l = l_run[h];
-            l += __shfl_xor_sync(0xffffffffu, l, 1);
-            l += __shfl_xor_sync(0xffffffffu, l, 2);
-            const float inv = 1.f / l;
             const int qrow = q0 + wg * (BQ / 2) + r + 8 * h;
-            if (qrow >= p.T) continue;
-            __half* orow = p.out + (long long)qrow * p.ldo + (long long)head * p.d;
-#pragma unroll
-            for (int ch = 0; ch < NCH; ch++)
-#pragma unroll
-                for (int c = 0; c < 8; c++) {
-                    const int col = 64 * ch + 8 * c + cq;
-                    if (col < p.d)     // d % 8 == 0: the pair is inside
-                        *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
-                }
+            rows[h] = qrow < p.T ? p.out + (long long)qrow * p.ldo + (long long)head * p.d : nullptr;
         }
+        fa_store(o, l_run, rows, p.d, cq);
     }
 }
 
-PFN_cuTensorMapEncodeTiled_v12000 fa_encode()
+// One launch of a flash kernel; the first launch of each kernel raises its dynamic shared-memory limit to smem.
+template <auto Kernel, typename... Args>
+int fa_launch_kernel(dim3 grid, int threads, int smem, cudaStream_t st, const Args&... args)
 {
-    static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = (PFN_cuTensorMapEncodeTiled_v12000)p;
-    });
-    return fn;
-}
-
-// [rows, heads*d] projection viewed as (d, heads, rows): strides (d*2, ld*2) bytes; box (64, 1, box_rows)
-bool head_map(CUtensorMap* map, const void* base, int d, int heads, int64_t rows, int64_t ld, uint32_t box_rows)
-{
-    auto enc = fa_encode();
-    if (!enc) return false;
-    cuuint64_t dims[3] = { (cuuint64_t)d, (cuuint64_t)heads, (cuuint64_t)rows };
-    cuuint64_t strides[2] = { (cuuint64_t)d * 2, (cuuint64_t)ld * 2 };
-    cuuint32_t box[3] = { 64, 1, box_rows };
-    cuuint32_t estr[3] = { 1, 1, 1 };
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e != cudaSuccess) return (int)e;
+        attr = true;
+    }
+    osb_launch(Kernel, grid, threads, (size_t)smem, st, args...);
+    return launched(1);
 }
 
 // ---- grouped-KV masked attention (ScaledDotProductAttention: prompt prefill) ----------------------------------------------------------
@@ -353,16 +383,8 @@ bool head_map(CUtensorMap* map, const void* base, int d, int heads, int64_t rows
 // chunks of the head dim (1: d <= 64, 2: 64 < d <= 128), BK = keys per tile.  At d = 128 the O accumulator is 64 fp32 registers per
 // thread, so that instantiation takes 64-key tiles (a 32-register score tile) to stay inside the 168 registers of a 384-thread CTA.
 // Masked keys keep their finite logit s*scale + mask (a row whose keys are all masked gets the softmax of those logits, as the
-// reference computes it); keys past Tk are padding (zero-filled by TMA) and get probability 0.
-template <int NCH, int BK>
-struct SdpaCfg {
-    static constexpr int Q_CHUNK = BQ * 128;            // 128 rows x 64 fp16 columns (one 128-byte swizzle row each)
-    static constexpr int KV_CHUNK = BK * 128;
-    static constexpr int Q_BYTES = NCH * Q_CHUNK;
-    static constexpr int KV_BYTES = NCH * KV_CHUNK;     // one K (or V) tile
-    static constexpr int SMEM = Q_BYTES + KV_STAGES * 2 * KV_BYTES + 1024 + 256;
-};
-
+// reference computes it); keys past Tk are padding (zero-filled by TMA) and get probability 0.  Q K^T runs over the whole of each
+// 64-column chunk (QKS = 4 NCH).
 struct SdpaParams {
     int rows;                // G * Tq: packed query rows per KV head
     int Tq, Tk, d;
@@ -389,36 +411,19 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
 sdpa_flash_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
                   const SdpaParams p)
 {
-    using C = SdpaCfg<NCH, BK>;
+    using C = FaCfg<NCH, BK, 4 * NCH>;
     constexpr float LOG2E = 1.4426950408889634f;
     osb_pdl_trigger_entry();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int r0 = blockIdx.x * BQ, hk = blockIdx.y;
+    const int n_kv = p.kv_tiles;
+    uint8_t* smem = fa_prologue(&map_q, &map_k, &map_v, C::BARS, FA_CONSUMERS, KV_STAGES);   // kv_empty: one arrival per consumer thread
     uint8_t* sQ = smem;
     uint8_t* sK = sQ + C::Q_BYTES;
     uint8_t* sV = sK + KV_STAGES * C::KV_BYTES;
-    uint64_t* bars = (uint64_t*)(sV + KV_STAGES * C::KV_BYTES);
-    uint64_t* q_full = bars;                           // [1]
-    uint64_t* kv_full = bars + 1;                      // [KV_STAGES]
+    uint64_t* q_full = (uint64_t*)(smem + C::BARS);   // [1]
+    uint64_t* kv_full = q_full + 1;                    // [KV_STAGES]
     uint64_t* kv_empty = kv_full + KV_STAGES;          // [KV_STAGES]
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int r0 = blockIdx.x * BQ, hk = blockIdx.y;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        mbar_init(q_full, 1);
-        for (int i = 0; i < KV_STAGES; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], FA_CONSUMERS); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    osb_pdl_wait();
-
-    const int n_kv = p.kv_tiles;
 
     if (warp == 0) {
         if (elect_one()) {
@@ -427,20 +432,13 @@ sdpa_flash_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
             for (int c = 0; c < NCH; c++) tma_load_3d(sQ + c * C::Q_CHUNK, &map_q, q_full, 64 * c, r0, hk);
         }
         __syncwarp();
-        for (int j = 0; j < n_kv; j++) {
-            const int st = j % KV_STAGES;
-            mbar_wait(&kv_empty[st], ((j / KV_STAGES) & 1) ^ 1);
-            if (elect_one()) {
-                mbar_expect_tx(&kv_full[st], 2 * C::KV_BYTES);
+        fa_produce_kv<KV_STAGES>(kv_full, kv_empty, n_kv, 2 * C::KV_BYTES, [&](int st, int j, uint64_t* bar) {
 #pragma unroll
-                for (int c = 0; c < NCH; c++) {
-                    tma_load_3d(sK + st * C::KV_BYTES + c * C::KV_CHUNK, &map_k, &kv_full[st], 64 * c, j * BK, hk);
-                    tma_load_3d(sV + st * C::KV_BYTES + c * C::KV_CHUNK, &map_v, &kv_full[st], 64 * c, j * BK, hk);
-                }
+            for (int c = 0; c < NCH; c++) {
+                tma_load_3d(sK + st * C::KV_BYTES + c * C::KV_CHUNK, &map_k, bar, 64 * c, j * BK, hk);
+                tma_load_3d(sV + st * C::KV_BYTES + c * C::KV_CHUNK, &map_v, bar, 64 * c, j * BK, hk);
             }
-            __syncwarp();
-        }
-        osb_pdl_trigger_late();
+        });
     } else if (warp >= 4) {
         // Fragments as in flash_attention_kernel: rows r, r + 8 of the warpgroup's 64; per 8-column block c the columns 8c + cq, + 1.
         const int wg = (warp >> 2) - 1;
@@ -469,14 +467,7 @@ sdpa_flash_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
             const int key0 = j * BK;
             mbar_wait(&kv_full[ks], (j / KV_STAGES) & 1);
             float s[BK / 2];
-#pragma unroll
-            for (int i = 0; i < BK / 2; i++) s[i] = 0.f;
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < NCH * 4; k++)
-                qk_mma<BK>(s, qdesc + (uint64_t)(((k >> 2) * C::Q_CHUNK >> 4) + (k & 3) * 2),
-                           kdesc0 + (uint64_t)((ks * C::KV_BYTES + (k >> 2) * C::KV_CHUNK) >> 4) + (uint64_t)((k & 3) * 2));
-            wgmma_commit();
+            fa_issue_qk<NCH, BK, 4 * NCH>(s, qdesc, kdesc0 + (uint64_t)(ks * C::KV_BYTES >> 4));
             // the mask loads (L2-resident: every head reads the same [Tq, Tk] block) are in flight while the MMAs run
             uint32_t mk[2][BK / 8];
 #pragma unroll
@@ -503,19 +494,13 @@ sdpa_flash_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
             float alpha[2], neg_m[2];
 #pragma unroll
             for (int h = 0; h < 2; h++) {
-                float mt = -INFINITY;
-#pragma unroll
-                for (int c = 0; c < BK / 8; c++) mt = fmaxf(mt, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
-                mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
-                mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
-                const float m_new = fmaxf(m_run[h], mt);
+                const float m_new = fmaxf(m_run[h], fa_row_max<BK>(s, h));
                 // m_new = -inf only when every logit so far is -inf (a -inf mask): keep the sums at 0 instead of producing NaN here
                 const bool none = m_new == -INFINITY;
                 alpha[h] = none ? 1.f : ex2_approx(m_run[h] - m_new);          // 0 on the first tile (m_run = -inf)
                 neg_m[h] = none ? 0.f : -m_new;
                 m_run[h] = m_new;
             }
-            uint32_t a[BK / 16][4];
             float lsum[2] = { 0.f, 0.f };
 #pragma unroll
             for (int c = 0; c < BK / 8; c++) {
@@ -524,101 +509,56 @@ sdpa_flash_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_consta
                     const float p0 = ex2_approx(s[4 * c + 2 * h] + neg_m[h]);
                     const float p1 = ex2_approx(s[4 * c + 2 * h + 1] + neg_m[h]);
                     lsum[h] += p0 + p1;
-                    a[c >> 1][(c & 1) * 2 + h] = pack_half2(p0, p1);
+                    s[4 * c + 2 * h] = p0; s[4 * c + 2 * h + 1] = p1;
                 }
             }
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-                l_run[h] = l_run[h] * alpha[h] + lsum[h];
-#pragma unroll
-                for (int ch = 0; ch < NCH; ch++)
-#pragma unroll
-                    for (int c = 0; c < 8; c++) { o[ch][4 * c + 2 * h] *= alpha[h]; o[ch][4 * c + 2 * h + 1] *= alpha[h]; }
-            }
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; kk++)
-#pragma unroll
-                for (int ch = 0; ch < NCH; ch++)
-                    wgmma_m64n64k16_f16_rs(o[ch], a[kk], vdesc0 + (uint64_t)((ks * C::KV_BYTES + ch * C::KV_CHUNK + kk * 2048) >> 4), 1u);
-            wgmma_commit();
+            for (int h = 0; h < 2; h++) l_run[h] = l_run[h] * alpha[h] + lsum[h];
+            uint32_t a[BK / 16][4];
+            fa_rescale_pack<NCH, BK>(o, a, s, alpha);
+            fa_issue_pv<NCH, BK, 4 * NCH>(o, a, vdesc0 + (uint64_t)(ks * C::KV_BYTES >> 4));
             wgmma_wait<0>();
             mbar_arrive(&kv_empty[ks]);
         }
-        // epilogue: O / l -> fp16 -> out[hk][R][col]
+        // out[hk][R][col]
+        __half* rows[2];
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-            float l = l_run[h];
-            l += __shfl_xor_sync(0xffffffffu, l, 1);
-            l += __shfl_xor_sync(0xffffffffu, l, 2);
-            const float inv = 1.f / l;
             const int R = r0 + wg * (BQ / 2) + r + 8 * h;
-            if (R >= p.rows) continue;
-            __half* orow = p.out + ((long long)hk * p.rows + R) * p.d;
-#pragma unroll
-            for (int ch = 0; ch < NCH; ch++)
-#pragma unroll
-                for (int c = 0; c < 8; c++) {
-                    const int col = 64 * ch + 8 * c + cq;
-                    if (col < p.d)     // d % 8 == 0: the pair is inside
-                        *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
-                }
+            rows[h] = R < p.rows ? p.out + ((long long)hk * p.rows + R) * p.d : nullptr;
         }
+        fa_store(o, l_run, rows, p.d, cq);
     }
 }
 
-// [heads, rows, d] contiguous viewed as (d, rows, heads); box (64, box_rows, 1)
-bool sdpa_map(CUtensorMap* map, const void* base, int d, int64_t rows, int64_t heads, uint32_t box_rows)
-{
-    auto enc = fa_encode();
-    if (!enc) return false;
-    cuuint64_t dims[3] = { (cuuint64_t)d, (cuuint64_t)rows, (cuuint64_t)heads };
-    cuuint64_t strides[2] = { (cuuint64_t)d * 2, (cuuint64_t)rows * d * 2 };
-    cuuint32_t box[3] = { 64, box_rows, 1 };
-    cuuint32_t estr[3] = { 1, 1, 1 };
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
+// q / k / v [Hkv, rows, d] contiguous viewed as (d, rows, Hkv); boxes (64, BQ or BK, 1)
 template <int NCH, int BK>
-int sdpa_launch(const void* q, const void* k, const void* v, const SdpaParams& p, int64_t Hkv, cudaStream_t st)
+int sdpa_launch(const void* q, const void* k, const void* v, SdpaParams p, int64_t Hkv, cudaStream_t st)
 {
-    using C = SdpaCfg<NCH, BK>;
+    using C = FaCfg<NCH, BK, 4 * NCH>;
+    const uint64_t d = p.d;
     CUtensorMap mq, mk, mv;
-    if (!sdpa_map(&mq, q, p.d, p.rows, Hkv, BQ) || !sdpa_map(&mk, k, p.d, p.Tk, Hkv, BK) || !sdpa_map(&mv, v, p.d, p.Tk, Hkv, BK))
+    if (!make_map(&mq, q, d, p.rows, Hkv, d * 2, p.rows * d * 2, 64, BQ, 1) || !make_map(&mk, k, d, p.Tk, Hkv, d * 2, p.Tk * d * 2, 64, BK, 1) ||
+        !make_map(&mv, v, d, p.Tk, Hkv, d * 2, p.Tk * d * 2, 64, BK, 1))
         return (int)cudaErrorInvalidValue;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(sdpa_flash_kernel<NCH, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
-        if (e != cudaSuccess) return (int)e;
-        attr = true;
-    }
-    SdpaParams pp = p;
-    pp.kv_tiles = (p.Tk + BK - 1) / BK;
+    p.kv_tiles = (p.Tk + BK - 1) / BK;
     dim3 grid((unsigned)((p.rows + BQ - 1) / BQ), (unsigned)Hkv);
-    osb_launch((sdpa_flash_kernel<NCH, BK>), grid, FA_THREADS, (size_t)C::SMEM, st, mq, mk, mv, pp);
-    return launched(1);
+    return fa_launch_kernel<sdpa_flash_kernel<NCH, BK>>(grid, FA_THREADS, C::SMEM, st, mq, mk, mv, p);
 }
 
-// K and V tensor maps take BK-row boxes, Q 128-row boxes; each box is 64 columns wide (one chunk)
+// q / k / v [rows, heads*d] (row strides ld*) viewed as (d, heads, rows); boxes (64, 1, BQ or BK)
 template <int NCH, int BK, int QKS>
 int fa_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, FaParams p, int64_t heads, cudaStream_t st)
 {
     using C = FaCfg<NCH, BK, QKS>;
+    const uint64_t d = p.d;
     CUtensorMap mq, mk, mv;
-    if (!head_map(&mq, q, p.d, (int)heads, p.T, ldq, BQ) || !head_map(&mk, k, p.d, (int)heads, p.Tk, ldk, BK) ||
-        !head_map(&mv, v, p.d, (int)heads, p.Tk, ldv, BK))
+    if (!make_map(&mq, q, d, heads, p.T, d * 2, ldq * 2, 64, 1, BQ) || !make_map(&mk, k, d, heads, p.Tk, d * 2, ldk * 2, 64, 1, BK) ||
+        !make_map(&mv, v, d, heads, p.Tk, d * 2, ldv * 2, 64, 1, BK))
         return (int)cudaErrorInvalidValue;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(flash_attention_kernel<NCH, BK, QKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
-        if (e != cudaSuccess) return (int)e;
-        attr = true;
-    }
     p.kv_tiles = (p.Tk + BK - 1) / BK;
     dim3 grid((unsigned)((p.T + BQ - 1) / BQ), (unsigned)heads);
-    osb_launch((flash_attention_kernel<NCH, BK, QKS>), grid, FA_THREADS, (size_t)C::SMEM, st, mq, mk, mv, p);
-    return launched(1);
+    return fa_launch_kernel<flash_attention_kernel<NCH, BK, QKS>>(grid, FA_THREADS, C::SMEM, st, mq, mk, mv, p);
 }
 
 // ---- wide heads: 160 < d <= 512 (the VAE's single-head d = 512 attention) --------------------------------------------------------------
@@ -644,7 +584,8 @@ constexpr int WD_Q_CHUNK = WD_BQ * 128;   // 64 rows x 64 fp16 columns
 constexpr int WD_K_CHUNK = WD_BK * 128;   // 64 keys x 64 columns of d (or 64 rows of d x 64 keys)
 constexpr int WD_V_CHUNK = WD_BK * 128;
 constexpr int WD_V_BYTES = WD_NV * WD_V_CHUNK;
-constexpr int WD_SMEM = WD_DCH * WD_Q_CHUNK + WD_K_STAGES * WD_K_CHUNK + WD_V_STAGES * WD_V_BYTES + 1024 + 256;
+constexpr int WD_BARS = WD_DCH * WD_Q_CHUNK + WD_K_STAGES * WD_K_CHUNK + WD_V_STAGES * WD_V_BYTES;
+constexpr int WD_SMEM = WD_BARS + 1024 + 256;
 
 // S (+)= Q_c K_c^T for one 64-column chunk c of d: 4 k-steps.  K-major K: 32 B per k-step inside the swizzle row; MN-major K^T (rows of
 // d): 16 rows of d = 2048 B per k-step.
@@ -681,18 +622,6 @@ flash_attention_wide_kernel(const __grid_constant__ CUtensorMap map_q, const __g
 {
     constexpr int KS = WD_K_STAGES, VS = WD_V_STAGES;
     osb_pdl_trigger_entry();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t* sQ = smem;
-    uint8_t* sK = sQ + WD_DCH * WD_Q_CHUNK;
-    uint8_t* sV = sK + KS * WD_K_CHUNK;
-    uint64_t* bars = (uint64_t*)(sV + VS * WD_V_BYTES);
-    uint64_t* q_full = bars;                           // [1]
-    uint64_t* k_full = bars + 1;                       // [KS]
-    uint64_t* k_empty = k_full + KS;                   // [KS]: one arrival per consumer warp
-    uint64_t* v_full = k_empty + KS;                   // [VS]
-    uint64_t* v_empty = v_full + VS;                   // [VS]
-
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // blockIdx.x = query tile * slices + slice: the slices of one query tile are adjacent, and x takes any T (y would stop at 65535 tiles)
     const int n_slices = (p.d + 64 * WD_NV - 1) / (64 * WD_NV);
@@ -700,21 +629,15 @@ flash_attention_wide_kernel(const __grid_constant__ CUtensorMap map_q, const __g
     const int q0 = (blockIdx.x / n_slices) * WD_BQ;
     const int head = blockIdx.y;
     const int n_dch = (p.d + 63) >> 6;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        mbar_init(q_full, 1);
-        for (int i = 0; i < KS; i++) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], WD_CONSUMERS / 32); }
-        for (int i = 0; i < VS; i++) { mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], WD_CONSUMERS / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    osb_pdl_wait();
-
+    uint8_t* smem = fa_prologue(&map_q, &map_k, &map_v, WD_BARS, WD_CONSUMERS / 32, KS, VS);
+    uint8_t* sQ = smem;
+    uint8_t* sK = sQ + WD_DCH * WD_Q_CHUNK;
+    uint8_t* sV = sK + KS * WD_K_CHUNK;
+    uint64_t* q_full = (uint64_t*)(smem + WD_BARS);   // [1]
+    uint64_t* k_full = q_full + 1;                     // [KS]
+    uint64_t* k_empty = k_full + KS;                   // [KS]: one arrival per consumer warp
+    uint64_t* v_full = k_empty + KS;                   // [VS]
+    uint64_t* v_empty = v_full + VS;                   // [VS]
     const int n_kv = p.kv_tiles;
 
     if (warp < 4) {
@@ -748,6 +671,7 @@ flash_attention_wide_kernel(const __grid_constant__ CUtensorMap map_q, const __g
                 }
                 __syncwarp();
             }
+            osb_pdl_trigger_late();
         }
     } else {
         // ===================== warpgroup 1: the CTA's 64 query rows =====================
@@ -799,47 +723,30 @@ flash_attention_wide_kernel(const __grid_constant__ CUtensorMap map_q, const __g
             __syncwarp();
             if (lane == 0) mbar_arrive(&v_empty[sv]);
         }
-        // epilogue: O / l -> fp16 -> out[head][q][col0 + c]
+        // out[head][q][col0 + c]
+        __half* rows[2];
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-            float l = l_run[h];
-            l += __shfl_xor_sync(0xffffffffu, l, 1);
-            l += __shfl_xor_sync(0xffffffffu, l, 2);
-            const float inv = 1.f / l;
             const int qrow = q0 + r + 8 * h;
-            if (qrow >= p.T) continue;
-            __half* orow = p.out + ((long long)head * p.T + qrow) * p.ldo + col0;
-#pragma unroll
-            for (int ch = 0; ch < WD_NV; ch++)
-#pragma unroll
-                for (int c = 0; c < 8; c++) {
-                    const int col = 64 * ch + 8 * c + cq;
-                    if (col0 + col < p.d)     // d % 8 == 0: the pair is inside
-                        *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
-                }
+            rows[h] = qrow < p.T ? p.out + ((long long)head * p.T + qrow) * p.ldo + col0 : nullptr;
         }
+        fa_store(o, l_run, rows, p.d - col0, cq);
     }
 }
 
 template <bool KT>
-int wd_launch(const void* q, const void* k, const void* v, const FaParams& p, int64_t heads, cudaStream_t st)
+int wd_launch(const void* q, const void* k, const void* v, FaParams p, int64_t heads, cudaStream_t st)
 {
     // q / v / out [heads, rows, d] viewed as (d, rows, heads); K^T [heads, d, Tk] as (Tk, d, heads) with 64 x 64 boxes
+    const uint64_t d = p.d, T = p.T, Tk = p.Tk;
     CUtensorMap mq, mk, mv;
-    const bool ok_k = KT ? sdpa_map(&mk, k, p.Tk, p.d, heads, 64) : sdpa_map(&mk, k, p.d, p.Tk, heads, WD_BK);
-    if (!sdpa_map(&mq, q, p.d, p.T, heads, WD_BQ) || !ok_k || !sdpa_map(&mv, v, p.d, p.Tk, heads, WD_BK)) return (int)cudaErrorInvalidValue;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(flash_attention_wide_kernel<KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, WD_SMEM);
-        if (e != cudaSuccess) return (int)e;
-        attr = true;
-    }
-    FaParams pp = p;
-    pp.kv_tiles = (p.Tk + WD_BK - 1) / WD_BK;
+    const bool ok_k = KT ? make_map(&mk, k, Tk, d, heads, Tk * 2, d * Tk * 2, 64, 64, 1) : make_map(&mk, k, d, Tk, heads, d * 2, Tk * d * 2, 64, WD_BK, 1);
+    if (!make_map(&mq, q, d, T, heads, d * 2, T * d * 2, 64, WD_BQ, 1) || !ok_k || !make_map(&mv, v, d, Tk, heads, d * 2, Tk * d * 2, 64, WD_BK, 1))
+        return (int)cudaErrorInvalidValue;
+    p.kv_tiles = (p.Tk + WD_BK - 1) / WD_BK;
     const int64_t n_slices = (p.d + 64 * WD_NV - 1) / (64 * WD_NV);
     dim3 grid((unsigned)((p.T + WD_BQ - 1) / WD_BQ * n_slices), (unsigned)heads);
-    osb_launch((flash_attention_wide_kernel<KT>), grid, WD_THREADS, (size_t)WD_SMEM, st, mq, mk, mv, pp);
-    return launched(1);
+    return fa_launch_kernel<flash_attention_wide_kernel<KT>>(grid, WD_THREADS, WD_SMEM, st, mq, mk, mv, p);
 }
 
 // ---- fp32 multi-head attention on the tensor cores: bf16 triple split --------------------------------------------------------------
@@ -855,17 +762,7 @@ int wd_launch(const void* q, const void* k, const void* v, const FaParams& p, in
 //   d <= 64:  64-key tiles, 2 stages: Q 48 KB + 2 x 48 KB;   registers O 32 + S 32 + P 3 x 16 + a P V chunk 32
 //   d <= 128: 32-key tiles, 2 stages: Q 96 KB + 2 x 48 KB;   O 64 + S 16 + P 3 x 8 + 32
 //   d <= 160: 32-key tiles, 1 stage:  Q 144 KB + 72 KB;      O 96 + S 16 + P 3 x 8 + 32
-template <int NCH, int BK, int QKS, int KS>
-struct F32xCfg {
-    static_assert(QKS <= 4 * NCH && (BK == 32 || BK == 64), "tile");
-    static constexpr int Q_CHUNK = BQ * 128;            // 128 rows x 64 bf16 columns
-    static constexpr int Q_PLANE = NCH * Q_CHUNK;
-    static constexpr int Q_BYTES = 3 * Q_PLANE;
-    static constexpr int KV_CHUNK = BK * 128;
-    static constexpr int KV_PLANE = NCH * KV_CHUNK;
-    static constexpr int KV_BYTES = 3 * KV_PLANE;       // one K (or V) tile: three planes
-    static constexpr int SMEM = Q_BYTES + KS * 2 * KV_BYTES + 1024 + 256;
-};
+// (FaCfg<NCH, BK, QKS, KS, 3>).
 
 // cross product x = 0..5 (hh, hm, mh, hl, lh, mm): plane of the A operand (Q, P) and of the B operand (K, V); 0 = h, 1 = m, 2 = l
 __host__ __device__ constexpr int x3a(int x) { return x == 2 || x == 5 ? 1 : (x == 4 ? 2 : 0); }
@@ -923,12 +820,7 @@ __device__ __forceinline__ void f32x_softmax(float (&s)[BK / 2], float (&m_run)[
     float m_new[2];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-        float mt = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < BK / 8; c++) mt = fmaxf(mt, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
-        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
-        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
-        m_new[h] = fmaxf(m_run[h], mt);
+        m_new[h] = fmaxf(m_run[h], fa_row_max<BK>(s, h));
         alpha[h] = expf(m_run[h] - m_new[h]);                        // 0 on the first tile (m_run = -inf)
         m_run[h] = m_new[h];
     }
@@ -959,36 +851,19 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
 flash_attention_f32x_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
                             const FaParams p, float scale, float* __restrict__ out)
 {
-    using C = F32xCfg<NCH, BK, QKS, KS>;
+    using C = FaCfg<NCH, BK, QKS, KS, 3>;
     osb_pdl_trigger_entry();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t* sQ = smem;
-    uint8_t* sK = sQ + C::Q_BYTES;
-    uint8_t* sV = sK + KS * C::KV_BYTES;
-    uint64_t* bars = (uint64_t*)(sV + KS * C::KV_BYTES);
-    uint64_t* q_full = bars;                           // [1]
-    uint64_t* kv_full = bars + 1;                      // [KS]
-    uint64_t* kv_empty = kv_full + KS;                 // [KS]: one arrival per consumer warp
-
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int head = blockIdx.y, heads = gridDim.y;
     const int q0 = blockIdx.x * BQ;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        mbar_init(q_full, 1);
-        for (int i = 0; i < KS; i++) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], FA_CONSUMERS / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    osb_pdl_wait();
-
     const int n_kv = p.kv_tiles;
+    uint8_t* smem = fa_prologue(&map_q, &map_k, &map_v, C::BARS, FA_CONSUMERS / 32, KS);   // kv_empty: one arrival per consumer warp
+    uint8_t* sQ = smem;
+    uint8_t* sK = sQ + C::Q_BYTES;
+    uint8_t* sV = sK + KS * C::KV_BYTES;
+    uint64_t* q_full = (uint64_t*)(smem + C::BARS);   // [1]
+    uint64_t* kv_full = q_full + 1;                    // [KS]
+    uint64_t* kv_empty = kv_full + KS;                 // [KS]
 
     if (warp < 4) {
         setmaxnreg_dec<FA_PRODUCER_REGS>();
@@ -1001,22 +876,16 @@ flash_attention_f32x_kernel(const __grid_constant__ CUtensorMap map_q, const __g
                     for (int c = 0; c < NCH; c++) tma_load_3d(sQ + pl * C::Q_PLANE + c * C::Q_CHUNK, &map_q, q_full, 64 * c, pl * heads + head, q0);
             }
             __syncwarp();
-            for (int j = 0; j < n_kv; j++) {
-                const int st = j % KS;
-                mbar_wait(&kv_empty[st], ((j / KS) & 1) ^ 1);
-                if (elect_one()) {
-                    mbar_expect_tx(&kv_full[st], 2 * C::KV_BYTES);
+            fa_produce_kv<KS>(kv_full, kv_empty, n_kv, 2 * C::KV_BYTES, [&](int st, int j, uint64_t* bar) {
 #pragma unroll
-                    for (int pl = 0; pl < 3; pl++)
+                for (int pl = 0; pl < 3; pl++)
 #pragma unroll
-                        for (int c = 0; c < NCH; c++) {
-                            const int off = st * C::KV_BYTES + pl * C::KV_PLANE + c * C::KV_CHUNK;
-                            tma_load_3d(sK + off, &map_k, &kv_full[st], 64 * c, pl * heads + head, j * BK);
-                            tma_load_3d(sV + off, &map_v, &kv_full[st], 64 * c, pl * heads + head, j * BK);
-                        }
-                }
-                __syncwarp();
-            }
+                    for (int c = 0; c < NCH; c++) {
+                        const int off = st * C::KV_BYTES + pl * C::KV_PLANE + c * C::KV_CHUNK;
+                        tma_load_3d(sK + off, &map_k, bar, 64 * c, pl * heads + head, j * BK);
+                        tma_load_3d(sV + off, &map_v, bar, 64 * c, pl * heads + head, j * BK);
+                    }
+            });
         }
     } else {
         // ===================== warpgroups 1, 2: 64 query rows each =====================
@@ -1101,78 +970,78 @@ flash_attention_f32x_kernel(const __grid_constant__ CUtensorMap map_q, const __g
             __syncwarp();
             if (lane == 0) mbar_arrive(&kv_empty[st]);
         }
-        // epilogue: O / l -> out[q, head*d + c] (fp32)
+        // out[q, head*d + c]
+        float* rows[2];
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-            float l = l_run[h];
-            l += __shfl_xor_sync(0xffffffffu, l, 1);
-            l += __shfl_xor_sync(0xffffffffu, l, 2);
-            const float inv = 1.f / l;
             const int qrow = q0 + wg * (BQ / 2) + r + 8 * h;
-            if (qrow >= p.T) continue;
-            float* orow = out + (long long)qrow * p.ldo + (long long)head * p.d;
-#pragma unroll
-            for (int ch = 0; ch < NCH; ch++)
-#pragma unroll
-                for (int c = 0; c < 8; c++) {
-                    const int col = 64 * ch + 8 * c + cq;
-                    if (col < p.d)     // d % 8 == 0: the pair is inside
-                        *reinterpret_cast<float2*>(orow + col) = make_float2(o[ch][4 * c + 2 * h] * inv, o[ch][4 * c + 2 * h + 1] * inv);
-                }
+            rows[h] = qrow < p.T ? out + (long long)qrow * p.ldo + (long long)head * p.d : nullptr;
         }
+        fa_store(o, l_run, rows, p.d, cq);
     }
 }
 
-// Every tensor map is made before anything is enqueued, so a refused launch enqueues nothing.  The plane buffers hold 2-byte elements
-// that the tensor maps only move: head_map's fp16 element type serves for bf16.
+// Every tensor map is made before anything is enqueued, so a refused launch enqueues nothing.  The plane buffers [rows][3][C] (plane p of
+// head h is "head" p * heads + h) hold 2-byte elements that the tensor maps only move: the fp16 element type serves for bf16.
 template <int NCH, int BK, int QKS, int KS>
 int f32x_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, float* out, FaParams p, float scale,
                 int64_t heads, __nv_bfloat16* planes, cudaStream_t st)
 {
-    using Cf = F32xCfg<NCH, BK, QKS, KS>;
+    using Cf = FaCfg<NCH, BK, QKS, KS, 3>;
     const int64_t C = heads * p.d;
+    const uint64_t d = p.d;
     __nv_bfloat16* pq = planes;
     __nv_bfloat16* pk = pq + 3 * p.T * C;
     __nv_bfloat16* pv = pk + 3 * p.Tk * C;
     CUtensorMap mq, mk, mv;
-    if (!head_map(&mq, pq, p.d, (int)(3 * heads), p.T, 3 * C, BQ) || !head_map(&mk, pk, p.d, (int)(3 * heads), p.Tk, 3 * C, BK) ||
-        !head_map(&mv, pv, p.d, (int)(3 * heads), p.Tk, 3 * C, BK))
+    if (!make_map(&mq, pq, d, 3 * heads, p.T, d * 2, 3 * C * 2, 64, 1, BQ) || !make_map(&mk, pk, d, 3 * heads, p.Tk, d * 2, 3 * C * 2, 64, 1, BK) ||
+        !make_map(&mv, pv, d, 3 * heads, p.Tk, d * 2, 3 * C * 2, 64, 1, BK))
         return (int)cudaErrorInvalidValue;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(flash_attention_f32x_kernel<NCH, BK, QKS, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cf::SMEM);
-        if (e != cudaSuccess) return (int)e;
-        attr = true;
-    }
     osb_launch((f32x_split_kernel), grid_for((size_t)((p.T + 2 * (int64_t)p.Tk) * C / 4), 256), 256, 0, st, q, ldq, k, ldk, v, ldv, pq, pk, pv,
                (int64_t)p.T, (int64_t)p.Tk, (int)C);
     const int e = launched();
     if (e) return e;
     p.kv_tiles = (p.Tk + BK - 1) / BK;
     dim3 grid((unsigned)((p.T + BQ - 1) / BQ), (unsigned)heads);
-    osb_launch((flash_attention_f32x_kernel<NCH, BK, QKS, KS>), grid, FA_THREADS, (size_t)Cf::SMEM, st, mq, mk, mv, p, scale, out);
-    return launched(1);
+    return fa_launch_kernel<flash_attention_f32x_kernel<NCH, BK, QKS, KS>>(grid, FA_THREADS, Cf::SMEM, st, mq, mk, mv, p, scale, out);
+}
+
+// 8 <= d <= 160, d % 8 == 0 (the 128-query kernels' head dims) and sequence lengths whose last query and key tiles start inside int32
+bool fa_dims_ok(int64_t T, int64_t Tk, int64_t d)
+{
+    return d >= 8 && d <= 160 && d % 8 == 0 && T >= 1 && Tk >= 1 && T <= (int64_t)INT32_MAX - BQ && Tk <= (int64_t)INT32_MAX - BKV;
+}
+
+// Launch rules of the flash entries whose softmax takes the running maximum over the raw scores: that is the maximum of the scaled
+// logits only for scale > 0 (and finite); heads are grid.y.
+bool fa_launch_ok(int64_t heads, float scale)
+{
+    return heads >= 1 && heads <= 65535 && scale > 0.f && scale < INFINITY;
+}
+
+bool aligned16(const void* a, const void* b, const void* c, const void* d, const void* e = nullptr)
+{
+    return (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c | (uintptr_t)d | (uintptr_t)e) & 15) == 0;
 }
 
 }  // namespace
 
 extern "C" int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
 {
-    return dtype == OSB_F16 && d >= 8 && d <= 160 && d % 8 == 0 && T >= 64 && Tk >= 1 && fa_encode() != nullptr;
+    return dtype == OSB_F16 && T >= 64 && fa_dims_ok(T, Tk, d) && get_encode() != nullptr;
 }
 
-// q [T, heads*d] (row stride ldq), k / v [Tk, heads*d] (row strides ldk / ldv), out [T, heads*d] (row stride ldo); fp16.
+// q [T, heads*d] (row stride ldq), k / v [Tk, heads*d] (row strides ldk / ldv), out [T, heads*d] (row stride ldo); fp16, 16-byte aligned.
+// scale > 0: the running maximum is taken over the raw scores.
 extern "C" int osb_flash_attention(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
                                    int64_t heads, int64_t T, int64_t Tk, int64_t d, float scale, void* stream)
 {
     if (heads * T == 0) return 0;
-    if (d < 8 || d > 160 || d % 8 || Tk < 1 || (ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 8)) return (int)cudaErrorInvalidValue;
-    if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) != 0) return (int)cudaErrorInvalidValue;
+    if (!fa_dims_ok(T, Tk, d) || !fa_launch_ok(heads, scale) || (ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 8) || !aligned16(q, k, v, out))
+        return (int)cudaErrorInvalidValue;
     FaParams p{};
     p.T = (int)T; p.Tk = (int)Tk; p.d = (int)d;
     p.scale_log2 = scale * 1.4426950408889634f;
-    static const float tau_env = [] { const char* e = getenv("OSB_FLASH_TAU"); float v = e ? (float)atof(e) : 0.f; return v < 0.f ? 0.f : (v > 12.f ? 12.f : v); }();
-    p.tau = tau_env;
     p.out = (__half*)out; p.ldo = ldo;
     cudaStream_t st = (cudaStream_t)stream;
     if (d <= 48) return fa_launch<1, 128, 3>(q, ldq, k, ldk, v, ldv, p, heads, st);
@@ -1184,8 +1053,7 @@ extern "C" int osb_flash_attention(const void* q, int64_t ldq, const void* k, in
 
 extern "C" int osb_flash_attention_f32x_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
 {
-    return dtype == OSB_F32 && d >= 8 && d <= 160 && d % 8 == 0 && T >= 1 && Tk >= 1 && T <= (int64_t)INT32_MAX - BQ && Tk <= (int64_t)INT32_MAX - BKV &&
-           fa_encode() != nullptr;
+    return dtype == OSB_F32 && fa_dims_ok(T, Tk, d) && get_encode() != nullptr;
 }
 
 // osb_flash_attention for fp32 q / k / v / out (row strides in floats, multiples of 4, >= heads * d; 16-byte aligned pointers), planes: scratch
@@ -1193,10 +1061,10 @@ extern "C" int osb_flash_attention_f32x_ok(int64_t T, int64_t Tk, int64_t d, int
 extern "C" int osb_flash_attention_f32x(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
                                         int64_t heads, int64_t T, int64_t Tk, int64_t d, float scale, void* planes, void* stream)
 {
-    if (!osb_flash_attention_f32x_ok(T, Tk, d, OSB_F32) || heads < 1 || heads > 65535 || !(scale > 0.f) || !(scale < INFINITY)) return (int)cudaErrorInvalidValue;
+    if (!osb_flash_attention_f32x_ok(T, Tk, d, OSB_F32) || !fa_launch_ok(heads, scale)) return (int)cudaErrorInvalidValue;
     const int64_t C = heads * d;
     if (ldq < C || ldk < C || ldv < C || ldo < C || (ldq % 4) || (ldk % 4) || (ldv % 4) || (ldo % 4) || C > INT32_MAX) return (int)cudaErrorInvalidValue;
-    if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out | (uintptr_t)planes) & 15) != 0) return (int)cudaErrorInvalidValue;
+    if (!aligned16(q, k, v, out, planes)) return (int)cudaErrorInvalidValue;
     FaParams p{};
     p.T = (int)T; p.Tk = (int)Tk; p.d = (int)d;
     p.out = nullptr; p.ldo = ldo;
@@ -1214,7 +1082,7 @@ extern "C" int osb_flash_attention_f32x(const void* q, int64_t ldq, const void* 
 extern "C" int osb_flash_attention_wide_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
 {
     return dtype == OSB_F16 && d > 160 && d <= 64 * WD_DCH && d % 8 == 0 && T >= 1 && Tk >= 1 && T <= (int64_t)INT32_MAX - WD_BQ &&
-           Tk <= (int64_t)INT32_MAX - WD_BK && fa_encode() != nullptr;
+           Tk <= (int64_t)INT32_MAX - WD_BK && get_encode() != nullptr;
 }
 
 // q [h, T, d], k [h, Tk, d] or (k_transposed) [h, d, Tk], v [h, Tk, d], out [h, T, d]; fp16, contiguous, 16-byte aligned.  K^T rows are
@@ -1223,13 +1091,11 @@ extern "C" int osb_flash_attention_wide_ok(int64_t T, int64_t Tk, int64_t d, int
 extern "C" int osb_flash_attention_wide(const void* q, const void* k, const void* v, void* out, int64_t heads, int64_t T, int64_t Tk, int64_t d,
                                         float scale, int k_transposed, int dtype, void* stream)
 {
-    if (!osb_flash_attention_wide_ok(T, Tk, d, dtype) || heads < 1 || heads > 65535 || (k_transposed && Tk % 8) || !(scale > 0.f) || !(scale < INFINITY))
+    if (!osb_flash_attention_wide_ok(T, Tk, d, dtype) || !fa_launch_ok(heads, scale) || (k_transposed && Tk % 8) || !aligned16(q, k, v, out))
         return (int)cudaErrorInvalidValue;
-    if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) != 0) return (int)cudaErrorInvalidValue;
     FaParams p{};
     p.T = (int)T; p.Tk = (int)Tk; p.d = (int)d;
     p.scale_log2 = scale * 1.4426950408889634f;
-    p.tau = 0.f;
     p.out = (__half*)out; p.ldo = d;
     cudaStream_t st = (cudaStream_t)stream;
     return k_transposed ? wd_launch<true>(q, k, v, p, heads, st) : wd_launch<false>(q, k, v, p, heads, st);
@@ -1238,16 +1104,17 @@ extern "C" int osb_flash_attention_wide(const void* q, const void* k, const void
 extern "C" int osb_sdpa_flash_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, int dtype)
 {
     return dtype == OSB_F16 && d == dv && d >= 8 && d <= 128 && d % 8 == 0 && Hkv >= 1 && Hkv <= 65535 && Hq >= Hkv && Hq % Hkv == 0 &&
-           Tq >= 1 && Tk >= 1 && (Hq / Hkv) * Tq <= (int64_t)INT32_MAX - BQ && Tk <= (int64_t)INT32_MAX - BKV && fa_encode() != nullptr;
+           Tq >= 1 && Tk >= 1 && (Hq / Hkv) * Tq <= (int64_t)INT32_MAX - BQ && Tk <= (int64_t)INT32_MAX - BKV && get_encode() != nullptr;
 }
 
-// q [Hq,Tq,d], k / v [Hkv,Tk,d], mask [Tq,Tk] (additive, may be null), out [Hq,Tq,d]; fp16, contiguous.
+// q [Hq,Tq,d], k / v [Hkv,Tk,d], mask [Tq,Tk] (additive, may be null), out [Hq,Tq,d]; fp16, contiguous.  Any scale: the running maximum
+// is taken over the scaled logits.
 extern "C" int osb_sdpa_flash(const void* q, const void* k, const void* v, const void* mask, void* out,
                               int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, float scale, void* stream)
 {
     if (Hq * Tq * d == 0) return 0;
     if (!osb_sdpa_flash_ok(Hq, Hkv, Tq, Tk, d, d, OSB_F16)) return (int)cudaErrorInvalidValue;
-    if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) != 0 || ((uintptr_t)mask & 3) != 0) return (int)cudaErrorInvalidValue;
+    if (!aligned16(q, k, v, out) || ((uintptr_t)mask & 3) != 0) return (int)cudaErrorInvalidValue;
     SdpaParams p{};
     p.rows = (int)((Hq / Hkv) * Tq); p.Tq = (int)Tq; p.Tk = (int)Tk; p.d = (int)d;
     p.scale_log2 = scale * 1.4426950408889634f;

@@ -95,10 +95,12 @@ struct Engine::Impl {
     // mha_prepass and fused_mha, which must agree on the K / V buffers
     bool mha_flash(int64_t T, int64_t Tk, int64_t d, DType ty, float scale) const
     {
-        if (!E.flash_attention || E.gemm_impl == 1) return false;
-        if (ty == DType::f32) return scale > 0.f && osb_flash_attention_f32x_ok(T, Tk, d, K(ty));
-        return osb_flash_attention_ok(T, Tk, d, K(ty));
+        // the flash kernels take the running maximum over the raw scores, which is the maximum of the scaled logits only for scale > 0
+        if (!flash_on() || !(scale > 0.f && scale < INFINITY)) return false;
+        return ty == DType::f32 ? osb_flash_attention_f32x_ok(T, Tk, d, K(ty)) : osb_flash_attention_ok(T, Tk, d, K(ty));
     }
+    // the flash attention kernels are on: b200_flash_attention, and not the CUDA-core GEMM path (b200_gemm_impl = 1)
+    bool flash_on() const { return E.flash_attention && E.gemm_impl != 1; }
 
     // int64 graph inputs and CUDA graphs: an op that consumes the host VALUES of such a tensor (other than through its device mirror)
     // makes the run un-capturable -- a replay would reuse the values of the captured run
@@ -1743,7 +1745,7 @@ void Engine::Impl::attention_core(const Tensor& q, const Tensor& k, const Tensor
     }
     // wide heads (the VAE's d = 512): one flash kernel, no [Tq, Tk] score buffer
     const bool aligned = (((uintptr_t)q.data() | (uintptr_t)k.data() | (uintptr_t)v.data() | (uintptr_t)out.data()) & 15) == 0;
-    if (!mask && dv == d && h <= 65535 && scale > 0.f && E.flash_attention && E.gemm_impl != 1 && aligned && osb_flash_attention_wide_ok(Tq, Tk, d, K(q.type))) {
+    if (!mask && dv == d && h <= 65535 && scale > 0.f && flash_on() && aligned && osb_flash_attention_wide_ok(Tq, Tk, d, K(q.type))) {
         // a transposed K with Tk % 8 != 0 (any odd latent) has rows of Tk * 2 bytes, which TMA cannot address: transpose it to
         // [h, Tk, d] (Tk * d scratch) and take the K-major kernel
         Tensor kk = k;
@@ -1853,7 +1855,8 @@ void Engine::Impl::mha_prepass(size_t si)
     if (xk.type != DType::f16 && xk.type != DType::f32) return;
     auto& qs = E.m_ops[i + 3].out[0].shape; auto& kts = E.m_ops[i + 8].out[0].shape;
     const int64_t h = qs[0], T = qs[1], d = qs[2], Tk = kts[2], C = h * d;
-    const float scale = ty == DType::f32 ? scalar_of(in(i + 14, 1), E.m_ops[i + 14]) : 1.f;     // only the fp32 kernel's rule reads it
+    float scale = scalar_of(in(i + 14, 1), E.m_ops[i + 14]);
+    if (ty == DType::f16) scale = __half2float(__float2half_rn(scale));     // as fused_mha rounds it
     const bool use_flash = mha_flash(T, Tk, d, ty, scale);
     const int64_t Tka = use_flash ? Tk : ((Tk + 7) & ~(int64_t)7);
     Tensor proxy; proxy.type = ty;      // only the dtype of the query side matters here
@@ -1961,7 +1964,7 @@ void Engine::Impl::fused_sdpa(const Step& s)
     Tensor o3 = out; o3.shape = { Hq, Tq, Dv };
     // prompt prefill (more query rows than the decode kernels take): one fused wgmma kernel for all the grouped heads
     const bool aligned = ((((uintptr_t)q.data() | (uintptr_t)k.data() | (uintptr_t)v.data() | (uintptr_t)out.data()) & 15) == 0) && (((uintptr_t)m.data() & 3) == 0);
-    if (q.type == DType::f16 && Tq > 16 && D == Dv && E.flash_attention && E.gemm_impl != 1 && aligned && osb_sdpa_flash_ok(Hq, Hkv, Tq, Tk, D, Dv, K(q.type))) {
+    if (q.type == DType::f16 && Tq > 16 && D == Dv && flash_on() && aligned && osb_sdpa_flash_ok(Hq, Hkv, Tq, Tk, D, Dv, K(q.type))) {
         ck(osb_sdpa_flash(q.data(), k.data(), v.data(), m.data(), out.mdata(), Hq, Hkv, Tq, Tk, D, scale, st), "osb_sdpa_flash");
         push(i + 5, 0, out);
         return;

@@ -1,11 +1,45 @@
 // tc_ptx.cuh -- inline-PTX wrappers shared by the sm_90a tensor-core kernels (gemm_wgmma.cu, attention_wgmma.cu): mbarrier, TMA,
-// shared-memory matrix descriptors and warpgroup MMA (wgmma).
+// shared-memory matrix descriptors and warpgroup MMA (wgmma); on the host, the TMA tensor maps they read through.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cstdio>
+#include <mutex>
 
 namespace tcptx {
+
+// ---- TMA tensor maps (host) ---------------------------------------------------------------------------------------
+
+// the driver's cuTensorMapEncodeTiled, or nullptr when the driver has none
+inline PFN_cuTensorMapEncodeTiled_v12000 get_encode()
+{
+    static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+            fn = (PFN_cuTensorMapEncodeTiled_v12000)p;
+    });
+    return fn;
+}
+
+// rank-3 fp16 tensor map with 128B swizzle; dims/strides innermost first
+inline bool make_map(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1_bytes, uint64_t s2_bytes,
+                     uint32_t b0, uint32_t b1, uint32_t b2, uint32_t traversal_stride = 1, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16)
+{
+    auto enc = get_encode();
+    if (!enc) return false;
+    cuuint64_t dims[3] = { d0, d1, d2 };
+    cuuint64_t strides[2] = { s1_bytes, s2_bytes };
+    cuuint32_t box[3] = { b0, b1, b2 };
+    cuuint32_t estr[3] = { 1, traversal_stride, traversal_stride };   // strided conv: every s-th pixel of the box span
+    CUresult r = enc(map, dtype, 3, const_cast<void*>(base), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------------------
 

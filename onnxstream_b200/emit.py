@@ -253,8 +253,8 @@ class GraphBuilder:
             r2 = self.node("Transpose", [r2], [(heads, d, t)], [("perm", "0,2,1")])
         return r2
 
-    def attention(self, x: T, ctx: T, heads: int) -> T:
-        """diffusers Attention: q from x, k/v from ctx; MatMul -> Mul(scale) -> Softmax -> MatMul; out proj with bias."""
+    def attention(self, x: T, ctx: T, heads: int, scale: Optional[float] = None) -> T:
+        """diffusers Attention: q from x, k/v from ctx; MatMul -> Mul(scale, default 1 / sqrt(d)) -> Softmax -> MatMul; out proj with bias."""
         _, t, c = x.shape
         tk = ctx.shape[1]
         d = c // heads
@@ -262,7 +262,7 @@ class GraphBuilder:
         k = self.split_heads(self.linear(ctx, c, bias=False), heads, transpose_k=True)
         v = self.split_heads(self.linear(ctx, c, bias=False), heads)
         s = self.node("MatMul", [q, k], [(heads, t, tk)])
-        s = self.node("Mul", [s, self.scalar(1.0 / math.sqrt(d))], [(heads, t, tk)])
+        s = self.node("Mul", [s, self.scalar(1.0 / math.sqrt(d) if scale is None else scale)], [(heads, t, tk)])
         p = self.node("Softmax", [s], [(heads, t, tk)], [("axis", "-1")])
         o = self.node("MatMul", [p, v], [(heads, t, d)])
         self.flops += 4 * heads * t * tk * d

@@ -91,6 +91,22 @@ def test_flash_attention_scope(K):
     assert K.osb_flash_attention(q.data_ptr(), 168, q.data_ptr(), 168, q.data_ptr(), 168, q.data_ptr(), 168, 1, 64, 64, 168, 1.0, _stream()) != 0
 
 
+def test_flash_attention_refuses_scales_it_cannot_compute(K):
+    """The kernel takes the running maximum over the raw scores times the scale, which is the maximum of the scaled logits only for
+    scale > 0: scale 0, a negative scale, inf and NaN are refused before anything is enqueued, and the output stays as it was."""
+    import torch
+    T, Tk, h, d = 128, 77, 2, 80
+    q, k, v = _inputs(T, Tk, h, d)
+    C = h * d
+    o = torch.full((T, C), 7.0, device="cuda", dtype=torch.half)
+    for scale in (0.0, -1.0, -1.0 / d ** 0.5, float("inf"), float("nan")):
+        n0 = K.osb_launch_count()
+        rc = K.osb_flash_attention(q.data_ptr(), C, k.data_ptr(), C, v.data_ptr(), C, o.data_ptr(), C, h, T, Tk, d, scale, _stream())
+        torch.cuda.synchronize()
+        assert rc != 0 and K.osb_launch_count() == n0, scale
+    assert bool((o == 7.0).all())
+
+
 @pytest.mark.parametrize("T,Tk,h,d", [(1024, 1024, 8, 40), (1024, 77, 8, 80), (256, 256, 8, 160)])
 def test_flash_attention_repeatable(K, T, Tk, h, d):
     """Two launches on the same inputs give the same bits."""
@@ -143,3 +159,41 @@ def test_unet_d80_d160_parity(engine_lib, oracle_lib, unet_d80_d160):
     off, _ = run_model(engine_lib, d, inputs, FP16, b200_options=(("b200_flash_attention", 0),))
     assert report(got[out], ref[out])["rel_to_max"] <= 3e-2, report(got[out], ref[out])
     assert report(got[out], off[out])["rel_to_max"] <= 1e-2, report(got[out], off[out])
+
+
+def test_engine_fp16_mha_negative_scale_keeps_the_chain(engine_lib):
+    """An fp16 multi-head attention block whose Mul scalar is -1 (d = 80).  On the flash kernel the running maximum would be the smallest
+    logit, and P = 2^(x - m) overflows fp16 once a row's logits spread over more than ~16 log2 units, as they do here.  The engine runs
+    the chain instead: as many tensor-core launches as with b200_flash_attention = 0, the same bits, finite, and softmax(-QK^T)V in fp64."""
+    import numpy as np
+    T, C, heads = 256, 160, 2
+    d = C // heads
+    x = np.random.default_rng(3).standard_normal((1, T, C), dtype=np.float32)
+    with tempfile.TemporaryDirectory(prefix="osb200_fa_neg_") as dirname:
+        g = emit.GraphBuilder(dirname + "/", "float16", 0, keep_in_memory=True)
+        xi = g.input("x", (1, T, C))
+        o = g.attention(xi, xi, heads, scale=-1.0)
+        g.mark_output(o)
+        g.finish()
+        res = {}
+        for flash in (1, 0):
+            got, m = run_model(engine_lib, dirname + "/", {"x": x}, FP16, b200_options=(("b200_flash_attention", flash),))
+            res[flash] = (np.asarray(got[o.name], dtype=np.float64), int(m.stats()["tc_launches"]))
+            m.close()
+    (on, tc_on), (off, tc_off) = res[1], res[0]
+    assert tc_on == tc_off, (tc_on, tc_off)
+    assert np.isfinite(on).all()
+    assert np.array_equal(on, off)
+    # fp64 on the fp16 input and weights: q / k / v projections (bias-free), per-head softmax(-q k^T) v, output projection with bias
+    blobs = [a for _, a in g.blobs.values() if a.dtype == np.float16]
+    wq, wk, wv, wo = [a.astype(np.float64) for a in blobs if a.ndim == 2]
+    bo = [a for a in blobs if a.ndim == 1 and a.size == C][-1].astype(np.float64)
+    xh = x[0].astype(np.float16).astype(np.float64)
+    qh, kh, vh = [(xh @ w).reshape(T, heads, d).transpose(1, 0, 2) for w in (wq, wk, wv)]
+    s = -(qh @ kh.transpose(0, 2, 1))
+    spread = (s.max(axis=-1) - s.min(axis=-1)).min() / np.log(2.0)
+    assert spread > 16, spread
+    p = np.exp(s - s.max(axis=-1, keepdims=True))
+    p /= p.sum(axis=-1, keepdims=True)
+    ref = (p @ vh).transpose(1, 0, 2).reshape(T, C) @ wo + bo
+    assert report(on.reshape(T, C), ref)["rel_to_max"] <= 3e-2, report(on.reshape(T, C), ref)
