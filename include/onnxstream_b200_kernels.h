@@ -219,6 +219,16 @@ int osb_flash_attention_wide_ok(int64_t T, int64_t Tk, int64_t d, int dtype);
 int osb_flash_attention_wide(const void* q, const void* k, const void* v, void* out, int64_t heads, int64_t T, int64_t Tk, int64_t d,
                              float scale, int k_transposed, int dtype, void* stream);
 
+/* osb_flash_attention_wide for fp32 (160 < d <= 512, d % 8 == 0) on the bf16 tensor cores at fp32 accuracy, with the numerics of
+ * osb_flash_attention_f32x: q, k and v are split into three bf16 planes each, Q K^T and P V sum the six significant cross products in
+ * fp32, the softmax is fp32 with an exact running maximum.  Same layouts as osb_flash_attention_wide with fp32 elements; a transposed K
+ * takes any Tk (the split transposes it).  `planes`: device scratch of 6 * (T + 2 * Tk) * heads * d bytes (16-byte aligned) for the bf16
+ * planes, written by the launch.  The launch returns cudaErrorInvalidValue and enqueues nothing for anything *_ok refuses, for misaligned
+ * pointers, for scale <= 0 or non-finite and for heads outside 1..65535.  osb_flash_attention_wide keeps refusing fp32. */
+int osb_flash_attention_wide_f32x_ok(int64_t T, int64_t Tk, int64_t d, int dtype);
+int osb_flash_attention_wide_f32x(const void* q, const void* k, const void* v, void* out, int64_t heads, int64_t T, int64_t Tk, int64_t d,
+                                  float scale, int k_transposed, void* planes, void* stream);
+
 /* Fused flash-style ScaledDotProductAttention on wgmma (fp16; d % 8 == 0, 8 <= d <= 128, dv == d): the prefill case of
  * src/onnxstream.cpp:7767-7882.  Semantics of osb_attention with k_transposed = 0: q [Hq,Tq,d], k / v [Hkv,Tk,d], additive mask
  * [Tq,Tk] (optional), out [Hq,Tq,d]; query head h reads KV head h / (Hq / Hkv).  The Hq / Hkv query heads of one KV head are

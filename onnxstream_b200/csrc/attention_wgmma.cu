@@ -18,6 +18,7 @@
 // llm.cpp's prompt prefill -- for d <= 128.
 // flash_attention_wide_kernel (below): 160 < d <= 512 -- the VAE decoder's single-head d = 512 attention -- with O split over its columns.
 // flash_attention_f32x_kernel (below): fp32 q / k / v / out on bf16 wgmma through the triple split, d <= 160.
+// flash_attention_wide_f32x_kernel (below): the wide kernel's slices with the f32x kernel's numerics, fp32 and 160 < d <= 512.
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -1024,6 +1025,249 @@ bool aligned16(const void* a, const void* b, const void* c, const void* d, const
     return (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c | (uintptr_t)d | (uintptr_t)e) & 15) == 0;
 }
 
+// ---- fp32 wide heads on the tensor cores: 160 < d <= 512 (the fp32 VAE decoder's single-head d = 512 attention) ---------------------
+// softmax(Q K^T * scale) V of flash_attention_wide_kernel for fp32 q [h, T, d], k [h, Tk, d] or [h, d, Tk], v [h, Tk, d], out [h, T, d],
+// with the numerics of flash_attention_f32x_kernel: bf16 planes x = h + m + l, six cross products, small ones first, f32x_softmax, P
+// split into three planes in registers, each tile's P V added to O in fp32.  Slices, grid and roles are those of the wide kernel (one CTA
+// per 256-column slice of V / O, 64-query tile and head; a TMA producer warp and one consumer warpgroup at 240 registers).
+// Planes: f32x_split_kernel writes q and v as [h * rows][3][d] (C = d); f32x_split_k_kernel writes K, either layout, K-major as
+// [h][3][Tk][d], so the kernel has one K layout.  Q / V are read through (3 d, rows, h) maps -- plane p's chunk c at column p d + 64 c, rows
+// past the head's last zero-filled; a chunk that ends past d reads the next plane's first columns, which meet K's zero-filled columns
+// (Q K^T) or feed output columns that are never stored (P V) -- and K through (d, Tk, 3 h).
+// Three planes of Q do not fit beside the rings (64 x 512 x 3 x 2 B = 192 KB), so Q streams with K: a stage of the Q K^T ring holds one
+// 64-column chunk of Q and of a 32-key K tile (3 x 8 KB + 3 x 4 KB); 3 stages (108 KB) + 2 stages of 32-key x 256-column V tiles (2 x
+// 48 KB) = 204 KB.  Registers: O 128 + S 16 + a chunk's product 16, then P 3 x 8 + a P V chunk 32.  Each chunk's six products go to a
+// fresh register tile that is added to S in fp32, so S, like O, never takes a tensor-core accumulation over more than one chunk.
+constexpr int WX_BK = 32;                               // keys per tile
+constexpr int WX_QK_STAGES = 3, WX_V_STAGES = 2;
+constexpr int WX_Q_PLANE = WD_BQ * 128;                 // one 64-column chunk of one plane: 64 rows x 128 B
+constexpr int WX_K_PLANE = WX_BK * 128;                 // 32 keys x 128 B
+constexpr int WX_QK_BYTES = 3 * WX_Q_PLANE + 3 * WX_K_PLANE;
+constexpr int WX_V_CHUNK = WX_BK * 128;                 // 32 keys x 64 columns of one plane
+constexpr int WX_V_PLANE = WD_NV * WX_V_CHUNK;
+constexpr int WX_V_BYTES = 3 * WX_V_PLANE;
+constexpr int WX_BARS = WX_QK_STAGES * WX_QK_BYTES + WX_V_STAGES * WX_V_BYTES;
+constexpr int WX_SMEM = WX_BARS + 1024 + 256;
+static_assert(WX_SMEM <= 227 * 1024, "shared memory");
+
+// k [h, Tk, d] (KT = false) or [h, d, Tk] (KT = true) fp32 -> bf16 planes pk [h][3][Tk][d]: a 32-key x 32-column tile through shared
+// memory, read along the input's contiguous axis and written along d
+template <bool KT>
+__global__ void __launch_bounds__(256) f32x_split_k_kernel(const float* __restrict__ k, __nv_bfloat16* __restrict__ pk, int Tk, int d)
+{
+    osb_pdl_prologue();
+    __shared__ float tile[32][33];     // [column][key]
+    const int key0 = blockIdx.x * 32, c0 = blockIdx.y * 32, head = blockIdx.z;
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    const float* src = k + (int64_t)head * Tk * d;
+    for (int i = ty; i < 32; i += 8) {
+        const int key = key0 + (KT ? tx : i), c = c0 + (KT ? i : tx);
+        if (key < Tk && c < d) tile[c - c0][key - key0] = KT ? src[(int64_t)c * Tk + key] : src[(int64_t)key * d + c];
+    }
+    __syncthreads();
+    __nv_bfloat16* dst = pk + (int64_t)head * 3 * Tk * d;
+    for (int i = ty; i < 32; i += 8) {
+        const int key = key0 + i, c = c0 + tx;
+        if (key < Tk && c < d) {
+            __nv_bfloat16 h, m, l;
+            bf16x3_split(tile[tx][i], h, m, l);
+            const int64_t o = (int64_t)key * d + c;
+            dst[o] = h;
+            dst[(int64_t)Tk * d + o] = m;
+            dst[2 * (int64_t)Tk * d + o] = l;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(WD_THREADS, 1)
+flash_attention_wide_f32x_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+                                 const __grid_constant__ CUtensorMap map_v, const FaParams p, float scale, float* __restrict__ out)
+{
+    constexpr int QS = WX_QK_STAGES, VS = WX_V_STAGES;
+    osb_pdl_trigger_entry();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    // blockIdx.x = query tile * slices + slice, as in flash_attention_wide_kernel
+    const int n_slices = (p.d + 64 * WD_NV - 1) / (64 * WD_NV);
+    const int col0 = (blockIdx.x % n_slices) * (64 * WD_NV);
+    const int q0 = (blockIdx.x / n_slices) * WD_BQ;
+    const int head = blockIdx.y;
+    const int n_dch = (p.d + 63) >> 6;
+    const int n_vch = min(WD_NV, (p.d - col0 + 63) >> 6);     // V / O chunks of this slice inside d
+    uint8_t* smem = fa_prologue(&map_q, &map_k, &map_v, WX_BARS, WD_CONSUMERS / 32, QS, VS);
+    uint8_t* sQK = smem;
+    uint8_t* sV = sQK + QS * WX_QK_BYTES;
+    uint64_t* qk_full = (uint64_t*)(smem + WX_BARS) + 1;    // [QS] (after fa_prologue's q_full, unused here)
+    uint64_t* qk_empty = qk_full + QS;                       // [QS]: one arrival per consumer warp
+    uint64_t* v_full = qk_empty + QS;                        // [VS]
+    uint64_t* v_empty = v_full + VS;                         // [VS]
+    const int n_kv = p.kv_tiles;
+
+    if (warp < 4) {
+        setmaxnreg_dec<WD_PRODUCER_REGS>();
+        if (warp == 0) {
+            int kc = 0;
+            for (int j = 0; j < n_kv; j++) {
+                for (int c = 0; c < n_dch; c++, kc++) {
+                    const int st = kc % QS;
+                    mbar_wait(&qk_empty[st], ((kc / QS) & 1) ^ 1);
+                    if (elect_one()) {
+                        uint8_t* s = sQK + st * WX_QK_BYTES;
+                        mbar_expect_tx(&qk_full[st], WX_QK_BYTES);
+                        for (int pl = 0; pl < 3; pl++) {
+                            tma_load_3d(s + pl * WX_Q_PLANE, &map_q, &qk_full[st], pl * p.d + 64 * c, q0, head);
+                            tma_load_3d(s + 3 * WX_Q_PLANE + pl * WX_K_PLANE, &map_k, &qk_full[st], 64 * c, j * WX_BK, 3 * head + pl);
+                        }
+                    }
+                    __syncwarp();
+                }
+                const int sv = j % VS;
+                mbar_wait(&v_empty[sv], ((j / VS) & 1) ^ 1);
+                if (elect_one()) {
+                    mbar_expect_tx(&v_full[sv], 3 * n_vch * WX_V_CHUNK);
+                    for (int pl = 0; pl < 3; pl++)
+                        for (int ch = 0; ch < n_vch; ch++)
+                            tma_load_3d(sV + sv * WX_V_BYTES + pl * WX_V_PLANE + ch * WX_V_CHUNK, &map_v, &v_full[sv], pl * p.d + col0 + 64 * ch,
+                                        j * WX_BK, head);
+                }
+                __syncwarp();
+            }
+            osb_pdl_trigger_late();
+        }
+    } else {
+        // ===================== warpgroup 1: the CTA's 64 query rows =====================
+        setmaxnreg_inc<WD_CONSUMER_REGS>();
+        const int r = (warp & 3) * 16 + (lane >> 2);
+        const int cq = 2 * (lane & 3);
+        // Q / K K-major (32 B per k-step inside the swizzle row), V MN-major (16 keys = 2048 B per k-step); 8-row groups 1024 B apart
+        const uint64_t qdesc0 = make_smem_desc(smem_u32(sQK), 16, 1024);
+        const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), WX_V_CHUNK, 1024);
+        float o[WD_NV][32];
+#pragma unroll
+        for (int ch = 0; ch < WD_NV; ch++)
+#pragma unroll
+            for (int i = 0; i < 32; i++) o[ch][i] = 0.f;
+        float m_run[2] = { -INFINITY, -INFINITY }, l_run[2] = { 0.f, 0.f }, alpha[2];
+        int kc = 0;
+        for (int j = 0; j < n_kv; j++) {
+            // S = sum over the chunks of d of the chunk's six cross products (small ones first, hh last; the first MMA overwrites t)
+            float s[WX_BK / 2];
+            for (int c = 0; c < n_dch; c++, kc++) {
+                const int st = kc % QS;
+                const uint64_t qdesc = qdesc0 + (uint64_t)((st * WX_QK_BYTES) >> 4);
+                const uint64_t kdesc = qdesc + (uint64_t)((3 * WX_Q_PLANE) >> 4);
+                mbar_wait(&qk_full[st], (kc / QS) & 1);
+                float t[WX_BK / 2];
+                fence_regs(t);
+                wgmma_fence();
+#pragma unroll
+                for (int xx = 0; xx < 6; xx++)
+#pragma unroll
+                    for (int k = 0; k < 4; k++) {
+                        const int x = 5 - xx;
+                        wgmma_m64n32k16_bf16<0>(t, qdesc + (uint64_t)(((x3a(x) * WX_Q_PLANE) >> 4) + k * 2),
+                                                kdesc + (uint64_t)(((x3b(x) * WX_K_PLANE) >> 4) + k * 2), (k | xx) != 0);
+                    }
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(t);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&qk_empty[st]);
+#pragma unroll
+                for (int i = 0; i < WX_BK / 2; i++) s[i] = c == 0 ? t[i] : s[i] + t[i];
+            }
+            f32x_softmax<WX_BK>(s, m_run, l_run, alpha, j * WX_BK, cq, p.Tk, scale);
+            // O *= alpha; P -> three bf16 planes in the A-fragment order of the P V MMA (see flash_attention_f32x_kernel)
+#pragma unroll
+            for (int ch = 0; ch < WD_NV; ch++)
+#pragma unroll
+                for (int c = 0; c < 8; c++)
+#pragma unroll
+                    for (int h = 0; h < 2; h++) { o[ch][4 * c + 2 * h] *= alpha[h]; o[ch][4 * c + 2 * h + 1] *= alpha[h]; }
+            uint32_t a[3][WX_BK / 16][4];
+#pragma unroll
+            for (int c = 0; c < WX_BK / 8; c++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    __nv_bfloat16 p0[3], p1[3];
+                    bf16x3_split(s[4 * c + 2 * h], p0[0], p0[1], p0[2]);
+                    bf16x3_split(s[4 * c + 2 * h + 1], p1[0], p1[1], p1[2]);
+#pragma unroll
+                    for (int pl = 0; pl < 3; pl++) a[pl][c >> 1][(c & 1) * 2 + h] = pack_bf162(p0[pl], p1[pl]);
+                }
+            // O_slice += P V_slice one 64-column chunk at a time, each through a fresh register tile added to O in fp32; chunks past d
+            // are neither loaded nor multiplied
+            const int sv = j % VS;
+            const uint64_t vdesc = vdesc0 + (uint64_t)((sv * WX_V_BYTES) >> 4);
+            mbar_wait(&v_full[sv], (j / VS) & 1);
+#pragma unroll
+            for (int pl = 0; pl < 3; pl++) fence_regs(a[pl]);
+#pragma unroll
+            for (int ch = 0; ch < WD_NV; ch++) {
+                if (ch >= n_vch) break;
+                float t[32];
+                fence_regs(t);
+                wgmma_fence();
+#pragma unroll
+                for (int xx = 0; xx < 6; xx++)
+#pragma unroll
+                    for (int kk = 0; kk < WX_BK / 16; kk++) {
+                        const int x = 5 - xx;
+                        wgmma_m64n64k16_bf16_rs(t, a[x3a(x)][kk], vdesc + (uint64_t)((x3b(x) * WX_V_PLANE + ch * WX_V_CHUNK + kk * 2048) >> 4),
+                                                (kk | xx) != 0);
+                    }
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(t);
+#pragma unroll
+                for (int i = 0; i < 32; i++) o[ch][i] += t[i];
+            }
+#pragma unroll
+            for (int pl = 0; pl < 3; pl++) fence_regs(a[pl]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&v_empty[sv]);
+        }
+        // out[head][q][col0 + c]
+        float* rows[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int qrow = q0 + r + 8 * h;
+            rows[h] = qrow < p.T ? out + ((long long)head * p.T + qrow) * p.d + col0 : nullptr;
+        }
+        fa_store(o, l_run, rows, p.d - col0, cq);
+    }
+}
+
+// Every tensor map is made before the splits are enqueued.  planes: pq [h * T][3][d], pk [h][3][Tk][d], pv [h * Tk][3][d].
+int wx_launch(const float* q, const float* k, const float* v, float* out, FaParams p, float scale, int64_t heads, bool kt,
+              __nv_bfloat16* planes, cudaStream_t st)
+{
+    const int64_t T = p.T, Tk = p.Tk, d = p.d;
+    __nv_bfloat16* pq = planes;
+    __nv_bfloat16* pk = pq + 3 * heads * T * d;
+    __nv_bfloat16* pv = pk + 3 * heads * Tk * d;
+    CUtensorMap mq, mk, mv;
+    if (!make_map(&mq, pq, 3 * d, T, heads, 3 * d * 2, T * 3 * d * 2, 64, WD_BQ, 1) ||
+        !make_map(&mk, pk, d, Tk, 3 * heads, d * 2, Tk * d * 2, 64, WX_BK, 1) ||
+        !make_map(&mv, pv, 3 * d, Tk, heads, 3 * d * 2, Tk * 3 * d * 2, 64, WX_BK, 1))
+        return (int)cudaErrorInvalidValue;
+    // q and v as [h * rows, d] with no K part, then K
+    osb_launch((f32x_split_kernel), grid_for((size_t)(heads * T * d / 4), 256), 256, 0, st, q, d, q, d, q, d, pq, pq, pq, heads * T,
+               (int64_t)0, (int)d);
+    int e = launched();
+    if (e) return e;
+    osb_launch((f32x_split_kernel), grid_for((size_t)(heads * Tk * d / 4), 256), 256, 0, st, v, d, v, d, v, d, pv, pv, pv, heads * Tk,
+               (int64_t)0, (int)d);
+    if ((e = launched())) return e;
+    const dim3 kgrid((unsigned)((Tk + 31) / 32), (unsigned)((d + 31) / 32), (unsigned)heads), kblock(32, 8);
+    if (kt) osb_launch((f32x_split_k_kernel<true>), kgrid, kblock, 0, st, k, pk, (int)Tk, (int)d);
+    else osb_launch((f32x_split_k_kernel<false>), kgrid, kblock, 0, st, k, pk, (int)Tk, (int)d);
+    if ((e = launched())) return e;
+    p.kv_tiles = (int)((Tk + WX_BK - 1) / WX_BK);
+    const int64_t n_slices = (d + 64 * WD_NV - 1) / (64 * WD_NV);
+    dim3 grid((unsigned)((T + WD_BQ - 1) / WD_BQ * n_slices), (unsigned)heads);
+    return fa_launch_kernel<flash_attention_wide_f32x_kernel>(grid, WD_THREADS, WX_SMEM, st, mq, mk, mv, p, scale, out);
+}
+
 }  // namespace
 
 extern "C" int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
@@ -1099,6 +1343,27 @@ extern "C" int osb_flash_attention_wide(const void* q, const void* k, const void
     p.out = (__half*)out; p.ldo = d;
     cudaStream_t st = (cudaStream_t)stream;
     return k_transposed ? wd_launch<true>(q, k, v, p, heads, st) : wd_launch<false>(q, k, v, p, heads, st);
+}
+
+extern "C" int osb_flash_attention_wide_f32x_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
+{
+    return dtype == OSB_F32 && d > 160 && d <= 64 * WD_DCH && d % 8 == 0 && T >= 1 && Tk >= 1 && T <= (int64_t)INT32_MAX - WD_BQ &&
+           Tk <= (int64_t)INT32_MAX - WX_BK && get_encode() != nullptr;
+}
+
+// osb_flash_attention_wide for fp32 q / k / v / out (contiguous, 16-byte aligned) on the bf16 tensor cores at fp32 accuracy.  K^T is
+// transposed by the split, so any Tk takes either layout.  planes: scratch of 6 (T + 2 Tk) heads d bytes.  Four launches: the splits of q,
+// v and k, then the attention.
+extern "C" int osb_flash_attention_wide_f32x(const void* q, const void* k, const void* v, void* out, int64_t heads, int64_t T, int64_t Tk,
+                                             int64_t d, float scale, int k_transposed, void* planes, void* stream)
+{
+    if (!osb_flash_attention_wide_f32x_ok(T, Tk, d, OSB_F32) || !fa_launch_ok(heads, scale) || !aligned16(q, k, v, out, planes))
+        return (int)cudaErrorInvalidValue;
+    FaParams p{};
+    p.T = (int)T; p.Tk = (int)Tk; p.d = (int)d;
+    p.out = nullptr; p.ldo = d;
+    return wx_launch((const float*)q, (const float*)k, (const float*)v, (float*)out, p, scale, heads, k_transposed != 0, (__nv_bfloat16*)planes,
+                     (cudaStream_t)stream);
 }
 
 extern "C" int osb_sdpa_flash_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, int dtype)

@@ -21,6 +21,15 @@ Prints ONE JSON line: the card (name, power limit, max SM clock, read with an nv
           tiled: the SD VAE decoder (emit.VAEConfig(), 32 x 32 latent tiles: T = 1024 per tile, the shape where the kernel alone is
           slower than the chain) decoding a 64 x 64 latent as 9 batch siblings of one run (tiled_vae.py), b200_flash_attention on and
           off alternated; device ms per run (last_gpu_ms), median of --tiled-runs runs after 2 warm-up runs each.
+  vae --f32: the same shapes in fp32, ms per call for
+            flash  : osb_flash_attention_wide_f32x (bf16 triple split; the three plane-split launches included)
+            chain  : the fp32 chain: osb_gemm(QK^T) -> osb_softmax_scaled -> osb_gemm(PV) on the CUDA cores through an fp32 [T, Tk]
+                     buffer
+          TFLOP/s of algorithmic fp32 work (4*T*Tk*d / t); flash_mma_tflops counts the bf16 MMA work the kernel issues (six products in
+          Q K^T once per slice and in P V: 6*2*T*Tk*d*(slices + 1)); the chain's score bytes; max|flash - chain|.
+          tiled: the SD VAE decoder as above with fp16 weights and fp32 arithmetic (no options: SDXL's default decode).
+          whole: the same decoder built for 64 x 64 and 128 x 128 latents decoding untiled, on and off alternated, median device ms of
+          --tiled-runs runs after one warm-up run each, and each setting's activation high-water.
   trace : (--trace DIR) per-kernel-name GPU time of one eager SD 1.5 UNet step (64x64 latent, fp16, resident weights, no CUDA graph)
           and the attention share: flash_attention_kernel, softmax_scaled_* and the tensor-core GEMM launched right before and right
           after each softmax (the QK^T / PV pair) over all kernel and memset time.  The chrome trace is written to DIR.
@@ -241,22 +250,115 @@ def vae_level(iters, warmup):
     return out
 
 
-def tiled_level(runs):
+def vae_level_f32(iters, warmup):
+    import torch
+    lib = ctypes.CDLL(ENGINE_LIB)
+    vp, i64, cf, ci = ctypes.c_void_p, ctypes.c_int64, ctypes.c_float, ctypes.c_int
+    lib.osb_flash_attention_wide_f32x.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64, cf, ci, vp, vp]
+    lib.osb_gemm.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i64, i64, i64, i64, ci, ci, ci, vp]
+    lib.osb_softmax_scaled.argtypes = [vp, vp, ci, i64, i64, cf, vp, i64, vp]
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    d, out = 512, []
+    for name, T in VAE_SHAPES:
+        Tk = T
+        g = torch.Generator(device="cuda").manual_seed(T + d)
+        q = torch.randn(T, d, device="cuda", generator=g)
+        kt = torch.randn(d, Tk, device="cuda", generator=g)
+        v = torch.randn(Tk, d, device="cuda", generator=g)
+        S = torch.empty(T, Tk, device="cuda")
+        planes = torch.empty(3 * (T + 2 * Tk) * d, device="cuda", dtype=torch.bfloat16)
+        o_flash = torch.zeros(T, d, device="cuda")
+        o_chain = torch.zeros(T, d, device="cuda")
+        scale = 1.0 / d ** 0.5
+
+        def flash():
+            assert lib.osb_flash_attention_wide_f32x(q.data_ptr(), kt.data_ptr(), v.data_ptr(), o_flash.data_ptr(), 1, T, Tk, d, scale, 1,
+                                                     planes.data_ptr(), stream) == 0
+
+        def chain():
+            assert lib.osb_gemm(q.data_ptr(), kt.data_ptr(), S.data_ptr(), None, None, 1, T, Tk, d, T * d, Tk * d, T * Tk, 0, F32, 0, stream) == 0
+            assert lib.osb_softmax_scaled(S.data_ptr(), S.data_ptr(), F32, T, Tk, scale, None, T, stream) == 0
+            assert lib.osb_gemm(S.data_ptr(), v.data_ptr(), o_chain.data_ptr(), None, None, 1, T, d, Tk, T * Tk, Tk * d, T * d, 0, F32, 0, stream) == 0
+
+        def timed(fn):
+            for _ in range(warmup):
+                fn()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(iters):
+                fn()
+            e1.record()
+            torch.cuda.synchronize()
+            return e0.elapsed_time(e1) / iters
+
+        t_flash, t_chain = timed(flash), timed(chain)
+        flop = 4.0 * T * Tk * d
+        slices = -(-d // 256)
+        out.append({"shape": name, "h": 1, "T": T, "Tk": Tk, "d": d, "flash_ms": round(t_flash, 4), "chain_ms": round(t_chain, 4),
+                    "flash_tflops": round(flop / t_flash / 1e9, 2), "chain_tflops": round(flop / t_chain / 1e9, 2),
+                    "flash_mma_tflops": round(6 * 2.0 * T * Tk * d * (slices + 1) / t_flash / 1e9, 2),
+                    "flash_vs_chain": round(t_chain / t_flash, 2), "chain_score_bytes": T * Tk * 4,
+                    "max_abs_diff": float((o_flash - o_chain).abs().max())})
+        del q, kt, v, S, planes, o_flash, o_chain
+        torch.cuda.empty_cache()
+    return out
+
+
+def _vae_models(d, f32):
+    """The decoder in d on b200_flash_attention 1 and 0: fp16 arithmetic, or (f32) fp32 arithmetic on the fp16 weights."""
+    models = {}
+    for flash in (1, 0):
+        m = Model(ENGINE_LIB, 0, "ram+nocache")
+        for o in (() if f32 else ("use_fp16_arithmetic", "fuse_ops_in_attention")):
+            m.set_option(o, True)
+        m.lib.model_set_option(m.h, b"b200_resident_weights", 1)
+        m.lib.model_set_option(m.h, b"b200_flash_attention", flash)
+        m.read_file(d + "model.txt")
+        models[flash] = m
+    return models
+
+
+def whole_level(runs):
+    import numpy as np
+    res = []
+    for latent in (64, 128):
+        d = tempfile.mkdtemp(prefix="osb200_attn_whole_") + "/"
+        try:
+            emit.emit_vae_decoder(d, emit.VAEConfig(latent=latent), "float16")
+            x = np.random.default_rng(0).standard_normal((1, 4, latent, latent)).astype(np.float32)
+            models = _vae_models(d, True)
+            ms, imgs, hw = {1: [], 0: []}, {}, {}
+            for i in range(runs + 1):
+                for flash in (1, 0):
+                    m = models[flash]
+                    m.clear_tensors()
+                    m.add_tensor("input_2E_1", x)
+                    m.run()
+                    if i == runs:
+                        imgs[flash] = m.get_tensor("outsample")
+                    if i >= 1:
+                        ms[flash].append(m.stats()["last_gpu_ms"])
+            for f, m in models.items():
+                hw[f] = int(m.stats()["act_high_water_bytes"])
+                m.close()
+        finally:
+            shutil.rmtree(d, ignore_errors=True)
+        med = {f: float(np.median(v)) for f, v in ms.items()}
+        res.append({"latent": latent, "T": latent * latent, "flash_ms": round(med[1], 3), "chain_ms": round(med[0], 3),
+                    "flash_runs_ms": [round(x, 3) for x in ms[1]], "chain_runs_ms": [round(x, 3) for x in ms[0]],
+                    "flash_act_high_water_mb": round(hw[1] / 2 ** 20, 1), "chain_act_high_water_mb": round(hw[0] / 2 ** 20, 1),
+                    "max_abs_diff": float(np.abs(imgs[1] - imgs[0]).max())})
+    return res
+
+
+def tiled_level(runs, f32=False):
     import numpy as np
     from onnxstream_b200 import tiled_vae as tv
     d = tempfile.mkdtemp(prefix="osb200_attn_tiled_") + "/"
     try:
         emit.emit_vae_decoder(d, emit.VAEConfig(latent=32), "float16")
         latent = np.random.default_rng(0).standard_normal((1, 4, 64, 64)).astype(np.float32)
-        models = {}
-        for flash in (1, 0):
-            m = Model(ENGINE_LIB, 0, "ram+nocache")
-            for o in ("use_fp16_arithmetic", "fuse_ops_in_attention"):
-                m.set_option(o, True)
-            m.lib.model_set_option(m.h, b"b200_resident_weights", 1)
-            m.lib.model_set_option(m.h, b"b200_flash_attention", flash)
-            m.read_file(d + "model.txt")
-            models[flash] = m
+        models = _vae_models(d, f32)
         ms, imgs, tiles = {1: [], 0: []}, {}, 0
         for i in range(runs + 2):
             for flash in (1, 0):
@@ -368,9 +470,11 @@ def main():
     c = card()
     res = {"card": c, "engine_lib": os.path.basename(ENGINE_LIB)}
     if a.vae:
-        res["vae"] = vae_level(a.iters, a.warmup)
+        res["vae"] = vae_level_f32(a.iters, a.warmup) if a.f32 else vae_level(a.iters, a.warmup)
         if a.tiled_runs:
-            res["tiled"] = tiled_level(a.tiled_runs)
+            res["tiled"] = tiled_level(a.tiled_runs, a.f32)
+            if a.f32:
+                res["whole"] = whole_level(a.tiled_runs)
     elif a.f32 and not a.skip_kernels:
         res["kernel"] = kernel_level_f32(a.iters, a.warmup)
     elif not a.skip_kernels:
