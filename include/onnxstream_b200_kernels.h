@@ -264,11 +264,18 @@ int osb_gemm_tc_eligible(int64_t M, int64_t N, int64_t K, int dtype);
  * eligible.  Tests and A/B runs. */
 void osb_tc_set_pair_mode(int mode);
 
+/* Tile shape and split-K factor of every later tensor-core GEMM / conv launch (fp16 operands; the fp32 path keeps 128 x 128).  0 in a field
+ * = the rule's choice for it; bm = -1: the previous rule for everything (128 x 128 tiles, split only below 100 tiles and from 32 k-blocks).
+ * A shape that has no instantiation for a launch's B layout and epilogue leaves that launch to the rule; a forced split is clamped to what
+ * the launch allows (no split with ldc != N, a residual that is not 8-byte aligned, Cout % 4 != 0, or no workspace).  Tests and A/B runs. */
+void osb_tc_set_tile(int bm, int bn, int split);
+
 /* Per-launch timing of the wgmma GEMM/conv kernel (CUDA events on the launching stream; eager mode only).
  * osb_tc_profile(1) starts recording, osb_tc_profile_read fills {launches, total ms, total FLOPs, total algorithmic bytes}. */
 void osb_tc_profile(int enable);
 int osb_tc_profile_read(double* out4);
-int osb_tc_profile_dump(char* buf, int cap);   /* one line per launch: M N K taps batch split conv ms gflop */
+int osb_tc_profile_dump(char* buf, int cap);   /* one line per launch: M N K taps batch split conv ms gflop bm bn kmajor
+                                                  (the tile, and 1 for a K-major B) */
 
 /* Programmatic dependent launch for every kernel of this library (default on). */
 int osb_pdl_enabled(void);

@@ -2,8 +2,10 @@
 //
 // One persistent, warp-specialised kernel, 384 threads:
 //   warpgroup 0      TMA producer: one warp issues cp.async.bulk.tensor tiles of A and B into 128B-swizzled shared memory, mbarrier-tracked
-//   warpgroups 1, 2  consumers: each issues wgmma (m64n128k16, fp32 accumulators in registers) for 64 rows of the 128 x 128 tile, then
-//                    runs the epilogue from its registers: add bias / residual, round to fp16, store
+//   warpgroups 1, 2  consumers: each issues wgmma (fp32 accumulators in registers) for its part of the BM x BN tile -- 64 rows at
+//                    BM = 128, half the columns at BM = 64 (TileCfg) -- then runs the epilogue from its registers: add bias /
+//                    residual, round to fp16, store
+// The tile shape and the split-K factor are chosen per launch (choose_tile: a cost model fit to measured times).
 // Shared memory holds a STAGES-deep ring of (A,B) k-blocks, so the producer is already fetching the next tile while the consumers run
 // the epilogue of this one.
 //
@@ -29,16 +31,30 @@
 
 namespace {
 
-constexpr int BLOCK_M = 128;
+constexpr int BLOCK_M = 128;           // the default tile, the uint8 kernel's and the CTA pairs' tile
 constexpr int BLOCK_N = 128;
 constexpr int BLOCK_K = 64;            // 64 fp16 = 128 bytes = one swizzle row
 constexpr int WG_K = 16;
-constexpr int STAGES = 6;
-constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KiB
-constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;  // 16 KiB
-constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * tcptx::GN_MAX_GROUPS * 4;
+constexpr int RING_BYTES = 6 * 32768;  // the (A, B) ring of every tile shape: 6 stages of the 128 x 128 tile
 constexpr int NUM_THREADS = 384;        // producer warpgroup + two consumer warpgroups
 constexpr int CONSUMER_THREADS = 256;
+
+// One tile shape, BM x BN.  BM = 128: consumer warpgroup wg owns rows [64 wg, 64 wg + 64) and all BN columns (m64nBN).  BM = 64: both
+// warpgroups share the 64 rows and split the columns, wg owns [wg BN/2, (wg + 1) BN/2) (m64n(BN/2)).  An MN-major B stage is BN/64 atoms of
+// 64 columns x 64 k-rows, so there BN (BM = 128) or BN/2 (BM = 64) is a multiple of 64.  The ring takes as many stages as fit RING_BYTES.
+template <int BM, int BN>
+struct TileCfg {
+    static constexpr int A_STAGE_BYTES = BM * BLOCK_K * 2;
+    static constexpr int B_STAGE_BYTES = BN * BLOCK_K * 2;
+    static constexpr int STAGES_FIT = RING_BYTES / (A_STAGE_BYTES + B_STAGE_BYTES);
+    static constexpr int STAGES = STAGES_FIT < 16 ? STAGES_FIT : 16;      // 2 * STAGES mbarriers in the 256-byte barrier area
+    static constexpr int WN = BM == 128 ? BN : BN / 2;                    // accumulator columns of one consumer warpgroup
+    static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * tcptx::GN_MAX_GROUPS * 4;
+    static_assert(BM == 64 || BM == 128, "BM");
+    static_assert(BN % 16 == 0 && B_STAGE_BYTES % 1024 == 0, "every stage and every warpgroup's B rows start on a 1024-byte swizzle boundary");
+};
+constexpr int A_STAGE_BYTES = TileCfg<BLOCK_M, BLOCK_N>::A_STAGE_BYTES;   // the uint8 kernel's stages (gemm_i8.cuh)
+constexpr int B_STAGE_BYTES = TileCfg<BLOCK_M, BLOCK_N>::B_STAGE_BYTES;
 
 struct TcParams {
     int M, N, K;                 // GEMM view of the problem (conv: M = Ho*Wo, K = Cin per tap)
@@ -68,35 +84,40 @@ struct TcParams {
     int f32_out;                 // raw fp32 accumulators go to `ws` even when split_k == 1; the reduce kernel writes fp32 C (+ fp32 bias / residual)
     long long stride_c;          // elements between batches
     long long ldc;               // elements between output rows (== N for a dense C)
+    int bm, bn;                  // the tile shape the launch runs (the kernel's template arguments; kept for the launch profile)
 };
 
 using namespace tcptx;
 
-// one k-block (64 elements of K) of a consumer warpgroup: 4 x m64n128k16
-template <int B_MN_MAJOR, bool BF16>
-__device__ __forceinline__ void mma_kblock(float (&acc)[64], uint64_t adesc, uint64_t bdesc)
+// one k-block (64 elements of K) of a consumer warpgroup: 4 x m64nWNk16
+template <int WN, int B_MN_MAJOR, bool BF16>
+__device__ __forceinline__ void mma_kblock(float (&acc)[WN / 2], uint64_t adesc, uint64_t bdesc)
 {
     constexpr uint32_t b_kstep = B_MN_MAJOR ? (WG_K * 128) >> 4 : (WG_K * 2) >> 4;   // descriptor address units (16 B)
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < BLOCK_K / WG_K; k++) {
         const uint64_t a = adesc + (uint64_t)(k * ((WG_K * 2) >> 4)), b = bdesc + (uint64_t)(k * b_kstep);
-        if (BF16) wgmma_m64n128k16_bf16<B_MN_MAJOR>(acc, a, b, 1u);
-        else wgmma_m64n128k16_f16<B_MN_MAJOR>(acc, a, b, 1u);
+        wgmma_ss<WN, B_MN_MAJOR, BF16>(acc, a, b, 1u);
     }
     wgmma_commit();
 }
 
 // ---- the kernel -----------------------------------------------------------------------------------------------
 
-// EXTRAS = the epilogue also adds `bias2` and gathers GroupNorm statistics.  A separate instantiation, so the common launches do not
-// carry the extra registers and code.  B_MN_MAJOR (== !p.b_kmajor) and BF16 (== p.bf16) are compile-time: the MMA loop has no branches.
-// PAIR = launched as clusters of two CTAs (see the top of the file); split_k == 1 and groups == 1 there.
-template <bool EXTRAS, int B_MN_MAJOR, bool BF16, bool PAIR>
+// BM x BN = the tile (TileCfg).  EXTRAS = the epilogue also adds `bias2` and gathers GroupNorm statistics.  A separate instantiation, so
+// the common launches do not carry the extra registers and code.  B_MN_MAJOR (== !p.b_kmajor) and BF16 (== p.bf16) are compile-time: the
+// MMA loop has no branches.  PAIR = launched as clusters of two CTAs (see the top of the file); 128 x 128 tiles, split_k == 1 and
+// groups == 1 there.
+template <int BM, int BN, bool EXTRAS, int B_MN_MAJOR, bool BF16, bool PAIR>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_b1,
                const __grid_constant__ CUtensorMap map_b2, const TcParams p)
 {
+    using Cfg = TileCfg<BM, BN>;
+    constexpr int STAGES = Cfg::STAGES, A_STAGE_BYTES = Cfg::A_STAGE_BYTES, B_STAGE_BYTES = Cfg::B_STAGE_BYTES, WN = Cfg::WN;
+    static_assert(!PAIR || (BM == 128 && BN == 128), "CTA pairs run 128 x 128 tiles");
+    static_assert(!B_MN_MAJOR || WN % 64 == 0, "an MN-major B is read in 64-column atoms");
     osb_pdl_trigger_entry();   // let the next kernel's CTAs be scheduled as ours drain; it waits for our completion before touching memory
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment for the 128B swizzle atoms
@@ -144,8 +165,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             int b = t2 / tiles_per_batch, r = t2 % tiles_per_batch;
             int mt = r % m_units, nt = r / m_units;
             if (PAIR) mt = 2 * mt + (int)rank;
-            int n0 = nt * BLOCK_N;
-            int y0 = 0, x0 = 0, m0 = mt * BLOCK_M;
+            int n0 = nt * BN;
+            int y0 = 0, x0 = 0, m0 = mt * BM;
             if (p.taps > 1 || p.bh > 0) { y0 = (mt / p.tiles_x) * p.bh; x0 = (mt % p.tiles_x) * p.bw; }
             // grouped launch: the batch index selects the B map; every operand is addressed at batch coordinate 0
             const CUtensorMap* mbp = &map_b;
@@ -182,13 +203,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         if (p.b_swap) tma_load_3d_s(sb, mbp, &full[stage], kglob, b, n0);
                         else tma_load_3d_s(sb, mbp, &full[stage], kglob, n0, b);
                     } else {
-                        // two 64-column atoms of 64 k-rows each
-                        if (p.b_swap) {
-                            tma_load_3d_s(sb, mbp, &full[stage], n0, b, kglob);
-                            tma_load_3d_s(sb + B_STAGE_BYTES / 2, mbp, &full[stage], n0 + 64, b, kglob);
-                        } else {
-                            tma_load_3d_s(sb, mbp, &full[stage], n0, kglob, b);
-                            tma_load_3d_s(sb + B_STAGE_BYTES / 2, mbp, &full[stage], n0 + 64, kglob, b);
+                        // BN/64 atoms of 64 columns x 64 k-rows
+#pragma unroll
+                        for (int at = 0; at < BN / 64; at++) {
+                            if (p.b_swap) tma_load_3d_s(sb + at * 8192, mbp, &full[stage], n0 + 64 * at, b, kglob);
+                            else tma_load_3d_s(sb + at * 8192, mbp, &full[stage], n0 + 64 * at, kglob, b);
                         }
                     }
                 }
@@ -200,16 +219,17 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         osb_pdl_trigger_late();   // every load of this CTA is issued: the next kernel may start its prologue on SMs that drain
     } else if (warp >= 4) {
         // ===================== consumers: MMA + epilogue (warpgroups 1 and 2) =====================
-        const int wg = (warp >> 2) - 1;          // rows [64 wg, 64 wg + 64) of the tile
+        const int wg = (warp >> 2) - 1;          // BM = 128: rows [64 wg, 64 wg + 64) of the tile; BM = 64: columns [WN wg, WN wg + WN)
         const int ct = (int)threadIdx.x - (NUM_THREADS - CONSUMER_THREADS);
+        const int wrow = BM == 128 ? 64 * wg : 0, wcol = BM == 128 ? 0 : WN * wg;
         // Descriptor templates: everything but the 14-bit start address is loop-invariant.
-        //   A, K-major SW128: 8-row groups 1024 B apart; K advances 32 B inside the swizzle row; warpgroup wg starts 64 rows (8 KiB) in.
-        //   B, K-major: same.  B, MN-major SW128: two 64-column atoms 8192 B apart (LBO), 8-row k-groups 1024 B apart (SBO);
-        //   K advances 16 rows = 2048 B.
-        const uint64_t adesc0 = make_smem_desc(smem_u32(smem_a) + wg * (BLOCK_M / 2) * 128, 16, 1024);
-        const uint64_t bdesc0 = p.b_kmajor ? make_smem_desc(smem_u32(smem_b), 16, 1024) : make_smem_desc(smem_u32(smem_b), B_STAGE_BYTES / 2, 1024);
+        //   A, K-major SW128: 8-row groups 1024 B apart; K advances 32 B inside the swizzle row; warpgroup wg starts wrow rows in.
+        //   B, K-major: same, starting wcol rows in.  B, MN-major SW128: 64-column atoms 8192 B apart (LBO), 8-row k-groups 1024 B apart
+        //   (SBO); K advances 16 rows = 2048 B; warpgroup wg starts wcol / 64 atoms in.
+        const uint64_t adesc0 = make_smem_desc(smem_u32(smem_a) + wrow * 128, 16, 1024);
+        const uint64_t bdesc0 = B_MN_MAJOR ? make_smem_desc(smem_u32(smem_b) + (wcol / 64) * 8192, 8192, 1024) : make_smem_desc(smem_u32(smem_b) + wcol * 128, 16, 1024);
         const bool partial = p.split_k > 1 || p.f32_out;
-        const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows of the tile: r_lo and r_lo + 8
+        const int r_lo = wrow + (warp & 3) * 16 + (lane >> 2);      // this thread's rows of the tile: r_lo and r_lo + 8
         const int cq = 2 * (lane & 3);                               // and its column pair inside every 8-column block
         auto release = [&](int s) {
             if (PAIR) {
@@ -225,18 +245,18 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             int b = t2 / tiles_per_batch, r = t2 % tiles_per_batch;
             int mt = r % m_units, nt = r / m_units;
             if (PAIR) mt = 2 * mt + (int)rank;      // past the last m-tile (odd count): no row is stored, the CTA still feeds its peer
-            const int n0 = nt * BLOCK_N;
-            const int n_end = min(p.N, n0 + BLOCK_N);
+            const int n0 = nt * BN, c0 = n0 + wcol;      // tile and warpgroup column origins
+            const int n_end = min(p.N, n0 + BN);
             const int kb_lo = sp * kb_per_split, kb_hi = min(kb_lo + kb_per_split, k_blocks_all);
 
-            float acc[64];
+            float acc[WN / 2];
 #pragma unroll
-            for (int i = 0; i < 64; i++) acc[i] = 0.f;
+            for (int i = 0; i < WN / 2; i++) acc[i] = 0.f;
             // one k-block of MMAs stays in flight: the stage of k-block kb-1 is released once the MMAs of kb are issued
             int prev = -1;
             for (int kb = kb_lo; kb < kb_hi; kb++) {
                 mbar_wait(&full[stage], phase);
-                mma_kblock<B_MN_MAJOR, BF16>(acc, adesc0 + (uint64_t)(stage * (A_STAGE_BYTES >> 4)), bdesc0 + (uint64_t)(stage * (B_STAGE_BYTES >> 4)));
+                mma_kblock<WN, B_MN_MAJOR, BF16>(acc, adesc0 + (uint64_t)(stage * (A_STAGE_BYTES >> 4)), bdesc0 + (uint64_t)(stage * (B_STAGE_BYTES >> 4)));
                 if (prev >= 0) { wgmma_wait<1>(); release(prev); }
                 prev = stage;
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -255,7 +275,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     row_ok[h] = y < p.Ho && x < p.Wo;
                     out_row[h] = (long long)y * p.Wo + x;
                 } else {
-                    int m = mt * BLOCK_M + row_in_tile;
+                    int m = mt * BM + row_in_tile;
                     row_ok[h] = m < p.M;
                     out_row[h] = m;
                 }
@@ -264,9 +284,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             if (p.groups > 1) cbase = b == 0 ? p.C : (b == 1 ? p.C1 : p.C2);    // stride_c == 0 in a grouped launch
             const bool pair_ok = (p.N & 1) == 0 && (p.ldc & 1) == 0;           // two adjacent columns move as one 4- / 8-byte vector
 #pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; j++) {
-                if (n0 + 8 * j >= n_end) break;     // warp-uniform
-                const int n = n0 + 8 * j + cq;
+            for (int j = 0; j < WN / 8; j++) {
+                if (c0 + 8 * j >= n_end) break;     // warp-uniform
+                const int n = c0 + 8 * j + cq;
                 const bool ok0 = n < n_end, ok1 = n + 1 < n_end;
                 float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;   // GroupNorm statistics of the two columns
                 float add0 = 0.f, add1 = 0.f;                   // per-column addends: bias (+ bias2)
@@ -371,26 +391,123 @@ constexpr size_t WS_MAX = OSB_WS_SPLITK_BYTES;   // fixed-capacity per-stream wo
 
 int num_sms();
 
-// pick a split factor: fill the SMs when the tile count is small, keep >= 2 k-blocks per split, stay inside the workspace
-int choose_split(int tiles, int k_blocks, size_t out_elems, cudaStream_t st, OsbWorkspace** ws_out)
+// The previous rule, kept selectable (osb_tc_set_tile(-1, 0, 0)) for A/B runs: 128 x 128 tiles, split K when there are fewer than 100 tiles
+// and at least 32 k-blocks, fill the SMs, keep >= 2 k-blocks per split, stay inside the workspace
+int old_split(int tiles, int k_blocks, size_t out_elems)
 {
-    static const int forced = [] { const char* e = getenv("OSB_TC_SPLIT"); return e ? atoi(e) : 0; }();   // tuning experiments only
-    // over the tensor-core shapes of the SD 1.5 UNet: below ~32 k-blocks the second launch (the reduce) costs more
-    // than the idle SMs do
-    *ws_out = nullptr;
-    static const int min_kb = [] { const char* e = getenv("OSB_TC_SPLIT_MINKB"); int v = e ? atoi(e) : 0; return v > 0 ? v : 32; }();
-    if ((tiles >= 100 && forced <= 0) || k_blocks < 4 || (k_blocks < min_kb && forced <= 0)) return 1;
-    int split = forced > 0 ? forced : num_sms() / tiles;
-    split = std::min(split, k_blocks / 2);
+    if (tiles >= 100 || k_blocks < 32) return 1;
+    int split = std::min(num_sms() / tiles, k_blocks / 2);
     while (split > 1 && (size_t)split * out_elems * 4 > WS_MAX) split--;
     if (split <= 1) return 1;
     int kb_per = (k_blocks + split - 1) / split;
-    split = (k_blocks + kb_per - 1) / kb_per;          // no empty splits: every CTA must run at least one k-block
+    return (k_blocks + kb_per - 1) / kb_per;          // no empty splits: every CTA must run at least one k-block
+}
+
+// ---- tile shapes and the rule that picks one per launch ------------------------------------------------------------------------------
+// The instantiated (BM, BN), each with the time one CTA takes for one k-block of it (ns; the cost model below).  K-major B (conv
+// weights, transposed GEMM weights) with and without EXTRAS; MN-major B ([K, N] MatMul weights) without.  The fp32 path (BF16) and CTA
+// pairs run 128 x 128 only.
+#define TC_TILES_KMAJOR(X) X(128, 128, 468.0) X(128, 64, 327.0) X(128, 80, 365.0) X(128, 160, 606.0) X(64, 64, 266.0) X(64, 128, 329.0) X(64, 160, 358.0)
+#define TC_TILES_MNMAJOR(X) X(128, 128, 499.0) X(128, 64, 284.0) X(64, 128, 300.0)
+struct TileShape { int bm, bn; double kb_ns; };
+#define TC_SHAPE(bm, bn, kb_ns) { bm, bn, kb_ns },
+const TileShape kTilesK[] = { TC_TILES_KMAJOR(TC_SHAPE) };
+const TileShape kTilesMN[] = { TC_TILES_MNMAJOR(TC_SHAPE) };
+#undef TC_SHAPE
+
+// forced by osb_tc_set_tile: 0 = the rule; g_tile_bm = -1: the previous rule (old_split) for every launch
+int g_tile_bm = 0, g_tile_bn = 0, g_tile_split = 0;
+
+// What the rule needs to know about a launch
+struct TileProblem {
+    int M, N;            // GEMM rows (per batch) and columns
+    int Ho, Wo;          // conv output (conv != 0): the tile's rows are a bw x bh box of pixels
+    int conv, batch, k_blocks, kmajor;
+    bool may_split;      // the epilogue and the workspace allow a split-K launch
+    bool only_128;       // the fp32 path: 128 x 128 tiles under the previous rule
+};
+struct TilePick { int bm, bn, split; };
+
+int conv_box_w(int bm, int Wo) { uint32_t r = 1; while ((int)r < Wo) r <<= 1; return std::min<int>(bm, (int)r); }
+int problem_m_tiles(const TileProblem& q, int bm)
+{
+    if (!q.conv) return (q.M + bm - 1) / bm;
+    const int bw = conv_box_w(bm, q.Wo), bh = bm / bw;
+    return ((q.Wo + bw - 1) / bw) * ((q.Ho + bh - 1) / bh);
+}
+
+// Cost model (ns), fit by least squares to the device times of the SD 1.5 UNet's tensor-core shapes under every tile on an H100 SXM
+// (scripts/tile_bench.py; DESIGN.md section 5):
+//   waves * (k-blocks per CTA * k-block time of the tile + WAVE_NS) + the reduce pass when split > 1.
+// Median error of the fit 7 %, 90th percentile 20 %.
+constexpr double WAVE_NS = 4500.0;         // per wave of CTAs: prologue, the first TMA round trip, the epilogue, the launch tail
+constexpr double REDUCE_NS = 4050.0;       // the reduce launch and its dependency
+constexpr double REDUCE_NS_PER_BYTE = 2.6e-5;   // the reduce's traffic: split fp32 planes read, fp16 output written
+
+double tile_cost(const TileProblem& q, const TileShape& t, int split)
+{
+    const long long ctas = (long long)problem_m_tiles(q, t.bm) * ((q.N + t.bn - 1) / t.bn) * q.batch * split;
+    const long long waves = (ctas + num_sms() - 1) / num_sms();
+    const int kb_cta = (q.k_blocks + split - 1) / split;
+    const double reduce_bytes = (double)q.batch * q.M * q.N * (4.0 * split + 2.0);
+    return (double)waves * (kb_cta * t.kb_ns + WAVE_NS) + (split > 1 ? REDUCE_NS + REDUCE_NS_PER_BYTE * reduce_bytes : 0.0);
+}
+
+// the split factors worth trying for one tile: none, or enough CTAs for one or two waves, each with >= 2 k-blocks and no empty split
+int split_for(const TileProblem& q, int tiles, int waves)
+{
+    if (!q.may_split || q.k_blocks < 4) return 1;
+    int split = std::min(waves * num_sms() / std::max(tiles, 1), q.k_blocks / 2);
+    while (split > 1 && (size_t)split * q.batch * q.M * q.N * 4 > WS_MAX) split--;
     if (split <= 1) return 1;
-    OsbWorkspace* ws = osb_workspace(st, OSB_WS_SPLITK);
-    if (!ws) return 1;                                  // capturing before any eager run, or out of memory: run unsplit
-    *ws_out = ws;
-    return split;
+    int kb_per = (q.k_blocks + split - 1) / split;
+    return (q.k_blocks + kb_per - 1) / kb_per;
+}
+
+TilePick choose_tile(const TileProblem& q)
+{
+    if (g_tile_bm < 0 || q.only_128) {
+        const int tiles = problem_m_tiles(q, BLOCK_M) * ((q.N + BLOCK_N - 1) / BLOCK_N) * q.batch;
+        return { BLOCK_M, BLOCK_N, q.may_split && q.k_blocks >= 4 ? old_split(tiles, q.k_blocks, (size_t)q.batch * q.M * q.N) : 1 };
+    }
+    const TileShape* shapes = q.kmajor ? kTilesK : kTilesMN;
+    const int n_shapes = q.kmajor ? (int)(sizeof(kTilesK) / sizeof(kTilesK[0])) : (int)(sizeof(kTilesMN) / sizeof(kTilesMN[0]));
+    // a forced shape without an instantiation for this B layout leaves the launch to the rule
+    bool forced_shape = false;
+    for (int i = 0; i < n_shapes; i++)
+        forced_shape |= (g_tile_bm > 0 || g_tile_bn > 0) && (g_tile_bm <= 0 || shapes[i].bm == g_tile_bm) && (g_tile_bn <= 0 || shapes[i].bn == g_tile_bn);
+    const bool forced_split = g_tile_split > 0 && (forced_shape || (g_tile_bm <= 0 && g_tile_bn <= 0));
+    TilePick best{ BLOCK_M, BLOCK_N, 1 };
+    double best_t = 1e300;
+    for (int i = 0; i < n_shapes; i++) {
+        const int bm = shapes[i].bm, bn = shapes[i].bn;
+        if (forced_shape && ((g_tile_bm > 0 && bm != g_tile_bm) || (g_tile_bn > 0 && bn != g_tile_bn))) continue;
+        const int tiles = problem_m_tiles(q, bm) * ((q.N + bn - 1) / bn) * q.batch;
+        int cand[3] = { 1, split_for(q, tiles, 1), split_for(q, tiles, 2) };
+        if (forced_split) {      // clamped to what the launch allows
+            int sp = q.may_split && q.k_blocks >= 2 ? std::min(g_tile_split, q.k_blocks) : 1;
+            while (sp > 1 && (size_t)sp * q.batch * q.M * q.N * 4 > WS_MAX) sp--;
+            if (sp > 1) { int kb_per = (q.k_blocks + sp - 1) / sp; sp = (q.k_blocks + kb_per - 1) / kb_per; }
+            cand[0] = cand[1] = cand[2] = std::max(sp, 1);
+        }
+        for (int sp : cand) {
+            const double t = tile_cost(q, shapes[i], sp);
+            if (t < best_t) { best_t = t; best = { bm, bn, sp }; }
+        }
+    }
+    return best;
+}
+
+// the pick, with the split-K workspace attached; no workspace (capturing before any eager run, or out of memory): the best unsplit pick
+TilePick choose_tile_ws(TileProblem q, cudaStream_t st, OsbWorkspace** ws_out)
+{
+    *ws_out = nullptr;
+    TilePick t = choose_tile(q);
+    if (t.split > 1) {
+        *ws_out = osb_workspace(st, OSB_WS_SPLITK);
+        if (!*ws_out) { q.may_split = false; t = choose_tile(q); }
+    }
+    return t;
 }
 
 // rank-3 map over (inner, row, batch) that keeps the global strides ascending: when the batch stride is the smaller one
@@ -414,7 +531,7 @@ int num_sms()
 }
 
 // optional per-launch timing (bench.py's roofline leg): CUDA events on the launching stream around every launch
-struct ProfRec { cudaEvent_t a, b; double flops, bytes; int M, N, K, taps, batch, split, conv; };
+struct ProfRec { cudaEvent_t a, b; double flops, bytes; int M, N, K, taps, batch, split, conv, bm, bn, kmajor; };
 bool g_prof = false;
 std::vector<ProfRec> g_prof_list;
 
@@ -429,10 +546,46 @@ void prof_begin(ProfRec& rec, const TcParams& p, cudaStream_t st)
     double a_bytes = (p.bh > 0 ? M * (p.K / kdiv) : M * Kt) * es * B;
     rec.bytes = a_bytes + N * Kt * es * (p.bh > 0 ? 1.0 : B) + M * N * es * B * (p.residual ? 2.0 : 1.0) + (p.bias ? N * es : 0.0);
     rec.M = p.M; rec.N = p.N; rec.K = p.K; rec.taps = p.taps; rec.batch = p.batch; rec.split = p.split_k; rec.conv = p.bh > 0;
+    rec.bm = p.bm; rec.bn = p.bn; rec.kmajor = p.b_kmajor;
     cudaEventRecord(rec.a, st);
 }
 
 using TcKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TcParams);
+
+// the instantiation, with its shared-memory limit raised once
+template <int BM, int BN, bool EXTRAS, int B_MN_MAJOR, bool BF16, bool PAIR>
+TcKernel ready_kernel(int* err)
+{
+    static const cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<BM, BN, EXTRAS, B_MN_MAJOR, BF16, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                      TileCfg<BM, BN>::SMEM_BYTES);
+    *err = (int)e;
+    return tc_gemm_kernel<BM, BN, EXTRAS, B_MN_MAJOR, BF16, PAIR>;
+}
+
+// the kernel for a launch; nullptr when (bm, bn) is not instantiated for its B layout / epilogue / type
+TcKernel pick_kernel(const TcParams& p, bool extras, bool pair, int* smem, int* err)
+{
+    *err = 0;
+    *smem = TileCfg<BLOCK_M, BLOCK_N>::SMEM_BYTES;
+    if (pair) {
+        if (p.bf16 || p.split_k != 1 || p.groups > 1 || p.bm != 128 || p.bn != 128) return nullptr;
+        return extras ? (p.b_kmajor ? ready_kernel<128, 128, true, 0, false, true>(err) : ready_kernel<128, 128, true, 1, false, true>(err))
+                      : (p.b_kmajor ? ready_kernel<128, 128, false, 0, false, true>(err) : ready_kernel<128, 128, false, 1, false, true>(err));
+    }
+    if (p.bf16) {   // the fp32 path: no bias2 / statistics
+        if (p.bm != 128 || p.bn != 128) return nullptr;
+        return p.b_kmajor ? ready_kernel<128, 128, false, 0, true, false>(err) : ready_kernel<128, 128, false, 1, true, false>(err);
+    }
+#define TC_PICK_K(M_, N_, COST_) \
+    if (p.bm == M_ && p.bn == N_) { *smem = TileCfg<M_, N_>::SMEM_BYTES; return extras ? ready_kernel<M_, N_, true, 0, false, false>(err) : ready_kernel<M_, N_, false, 0, false, false>(err); }
+#define TC_PICK_MN(M_, N_, COST_) \
+    if (p.bm == M_ && p.bn == N_) { *smem = TileCfg<M_, N_>::SMEM_BYTES; return ready_kernel<M_, N_, false, 1, false, false>(err); }
+    if (p.b_kmajor) { TC_TILES_KMAJOR(TC_PICK_K) }
+    else if (!extras) { TC_TILES_MNMAJOR(TC_PICK_MN) }
+#undef TC_PICK_K
+#undef TC_PICK_MN
+    return nullptr;
+}
 
 // pair: clusters of two CTAs sharing B (the B map's box covers half a tile: 64 rows K-major, one 64-column atom MN-major)
 int launch(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cudaStream_t st, const CUtensorMap* mb1p = nullptr, const CUtensorMap* mb2p = nullptr,
@@ -440,38 +593,18 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cuda
 {
     const CUtensorMap& mb1 = mb1p ? *mb1p : mb;
     const CUtensorMap& mb2 = mb2p ? *mb2p : mb;
-    static bool attr_set = false;
-    if (!attr_set) {
-        TcKernel kernels[] = {
-            tc_gemm_kernel<false, 0, false, false>, tc_gemm_kernel<false, 1, false, false>, tc_gemm_kernel<true, 0, false, false>, tc_gemm_kernel<true, 1, false, false>,
-            tc_gemm_kernel<false, 0, true, false>, tc_gemm_kernel<false, 1, true, false>,
-            tc_gemm_kernel<false, 0, false, true>, tc_gemm_kernel<false, 1, false, true>, tc_gemm_kernel<true, 0, false, true>, tc_gemm_kernel<true, 1, false, true> };
-        for (auto k : kernels) {
-            cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-            if (e != cudaSuccess) return (int)e;
-        }
-        attr_set = true;
-    }
     const bool extras = p.bias2 != nullptr || p.gn_stats != nullptr;
-    TcKernel k;
-    if (pair) {
-        if (p.bf16 || p.split_k != 1 || p.groups > 1) return (int)cudaErrorInvalidValue;
-        k = extras ? (p.b_kmajor ? tc_gemm_kernel<true, 0, false, true> : tc_gemm_kernel<true, 1, false, true>)
-                   : (p.b_kmajor ? tc_gemm_kernel<false, 0, false, true> : tc_gemm_kernel<false, 1, false, true>);
-    } else if (p.bf16) {   // the fp32 path: no bias2 / statistics
-        k = p.b_kmajor ? tc_gemm_kernel<false, 0, true, false> : tc_gemm_kernel<false, 1, true, false>;
-    } else if (extras) {
-        k = p.b_kmajor ? tc_gemm_kernel<true, 0, false, false> : tc_gemm_kernel<true, 1, false, false>;
-    } else {
-        k = p.b_kmajor ? tc_gemm_kernel<false, 0, false, false> : tc_gemm_kernel<false, 1, false, false>;
-    }
+    int smem = 0, err = 0;
+    TcKernel k = pick_kernel(p, extras, pair, &smem, &err);
+    if (err) return err;
+    if (!k) return (int)cudaErrorInvalidValue;
     int grid;
     if (pair) {
         // a persistent grid must be co-resident: clusters need both SMs in one GPC, so fewer than num_sms / 2 of them may fit at once
         static int max_clusters = 0;
         if (!max_clusters) {
             cudaLaunchConfig_t cfg{};
-            cfg.gridDim = dim3(2 * (num_sms() / 2)); cfg.blockDim = dim3(NUM_THREADS); cfg.dynamicSmemBytes = SMEM_BYTES;
+            cfg.gridDim = dim3(2 * (num_sms() / 2)); cfg.blockDim = dim3(NUM_THREADS); cfg.dynamicSmemBytes = smem;
             cudaLaunchAttribute attr[1];
             attr[0].id = cudaLaunchAttributeClusterDimension;
             attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
@@ -487,7 +620,7 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, cuda
     }
     ProfRec rec{};
     if (g_prof) prof_begin(rec, p, st);
-    osb_launch_cluster(k, grid, NUM_THREADS, (size_t)SMEM_BYTES, st, pair ? 2u : 1u, ma, mb, mb1, mb2, p);
+    osb_launch_cluster(k, grid, NUM_THREADS, (size_t)smem, st, pair ? 2u : 1u, ma, mb, mb1, mb2, p);
     if (p.f32_out) {
         launched(1);
         const long long total = (long long)p.batch * p.M * p.N;
@@ -538,6 +671,11 @@ bool use_pair(int64_t m_tiles, int64_t N)
 
 extern "C" void osb_tc_set_pair_mode(int mode) { g_pair_mode = mode; }
 
+extern "C" void osb_tc_set_tile(int bm, int bn, int split)
+{
+    g_tile_bm = bm; g_tile_bn = bm < 0 ? 0 : bn; g_tile_split = bm < 0 ? 0 : split;
+}
+
 extern "C" void osb_tc_profile(int enable)
 {
     for (auto& r : g_prof_list) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
@@ -559,14 +697,15 @@ extern "C" int osb_tc_profile_read(double* out4)
     return 0;
 }
 
-// One text line per recorded launch: "M N K taps batch split conv ms gflop"
+// One text line per recorded launch: "M N K taps batch split conv ms gflop bm bn kmajor"
 extern "C" int osb_tc_profile_dump(char* buf, int cap)
 {
     int off = 0;
     for (auto& r : g_prof_list) {
         float t = 0.f;
         if (cudaEventSynchronize(r.b) != cudaSuccess || cudaEventElapsedTime(&t, r.a, r.b) != cudaSuccess) return -1;
-        int n = snprintf(buf + off, cap - off, "%d %d %d %d %d %d %d %.4f %.3f\n", r.M, r.N, r.K, r.taps, r.batch, r.split, r.conv, t, r.flops * 1e-9);
+        int n = snprintf(buf + off, cap - off, "%d %d %d %d %d %d %d %.4f %.3f %d %d %d\n", r.M, r.N, r.K, r.taps, r.batch, r.split, r.conv, t, r.flops * 1e-9,
+                         r.bm, r.bn, r.kmajor);
         if (n < 0 || off + n >= cap) break;
         off += n;
     }
@@ -730,27 +869,30 @@ int osb_tc_gemm_launch(const void* A, const void* B, void* C, const void* bias, 
         }
         return 0;
     }
+    const int64_t k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
+    const bool pair = !g_f32x && use_pair((M + BLOCK_M - 1) / BLOCK_M, N);
+    // the split-K reduce reads the residual as 8-byte vectors: a residual that is not 8-byte aligned runs unsplit (scalar epilogue reads)
+    const bool split_ok = ldc == N && (sc == M * N || batch == 1) && ((uintptr_t)residual & 7) == 0;
+    TileProblem q{ (int)M, (int)N, 0, 0, 0, (int)batch, (int)k_blocks, bt ? 1 : 0, split_ok && !pair, g_f32x != 0 };
+    OsbWorkspace* wsp = nullptr;
+    const TilePick t = pair ? TilePick{ BLOCK_M, BLOCK_N, 1 } : choose_tile_ws(q, st, &wsp);
     int a_swap = 0, b_swap = 0;
-    if (!make_map_rb(&ma, A, (uint64_t)K, (uint64_t)M, abatch, (uint64_t)lda * 2, (uint64_t)(sa ? sa : M * lda) * 2, BLOCK_K, BLOCK_M, &a_swap)) return (int)cudaErrorInvalidValue;
-    int64_t m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-    const bool pair = !g_f32x && use_pair(m_tiles, N);
-    bool okb = bt ? make_map_rb(&mb, B, (uint64_t)K, (uint64_t)N, bbatch, (uint64_t)ldb * 2, (uint64_t)(sb ? sb : N * ldb) * 2, BLOCK_K, pair ? BLOCK_N / 2 : BLOCK_N, &b_swap)
+    if (!make_map_rb(&ma, A, (uint64_t)K, (uint64_t)M, abatch, (uint64_t)lda * 2, (uint64_t)(sa ? sa : M * lda) * 2, BLOCK_K, t.bm, &a_swap)) return (int)cudaErrorInvalidValue;
+    bool okb = bt ? make_map_rb(&mb, B, (uint64_t)K, (uint64_t)N, bbatch, (uint64_t)ldb * 2, (uint64_t)(sb ? sb : N * ldb) * 2, BLOCK_K, pair ? BLOCK_N / 2 : t.bn, &b_swap)
                   : make_map_rb(&mb, B, (uint64_t)N, (uint64_t)K, bbatch, (uint64_t)ldb * 2, (uint64_t)(sb ? sb : K * ldb) * 2, 64, BLOCK_K, &b_swap);
     if (!okb) return (int)cudaErrorInvalidValue;
     TcParams p{};
     p.M = (int)M; p.N = (int)N; p.K = (int)K; p.batch = (int)batch;
-    p.m_tiles = (int)m_tiles; p.n_tiles = (int)((N + BLOCK_N - 1) / BLOCK_N);
+    p.bm = t.bm; p.bn = t.bn;
+    p.m_tiles = (int)((M + t.bm - 1) / t.bm); p.n_tiles = (int)((N + t.bn - 1) / t.bn);
     p.b_kmajor = bt ? 1 : 0;
     p.a_swap = a_swap; p.b_swap = b_swap;
     p.taps = 1; p.kw = 1; p.bh = 0; p.bw = 0; p.tiles_x = 1;
-    p.k_blocks_per_tap = (int)((K + BLOCK_K - 1) / BLOCK_K);
+    p.k_blocks_per_tap = (int)k_blocks;
     p.stride = 1;
     p.C = (__half*)C; p.bias = (const __half*)bias; p.residual = (const __half*)residual; p.stride_c = sc; p.ldc = ldc;
-    if (pair) { p.split_k = 1; return launch(ma, mb, p, st, nullptr, nullptr, true); }
-    OsbWorkspace* wsp = nullptr;
-    // the split-K reduce reads the residual as 8-byte vectors: a residual that is not 8-byte aligned runs unsplit (scalar epilogue reads)
-    const bool split_ok = ldc == N && (sc == M * N || batch == 1) && ((uintptr_t)residual & 7) == 0;
-    p.split_k = split_ok ? choose_split(p.m_tiles * p.n_tiles * p.batch, p.k_blocks_per_tap, (size_t)batch * M * N, st, &wsp) : 1;
+    p.split_k = t.split;
+    if (pair) return launch(ma, mb, p, st, nullptr, nullptr, true);
     p.ws = wsp ? wsp->splitk : nullptr;
     if (g_f32x && !f32x_params(p, wsp, st)) return (int)cudaErrorNotSupported;
     return launch(ma, mb, p, st);
@@ -762,20 +904,22 @@ int osb_tc_gemm_grouped_launch(const void* A, const void* const* B, void* const*
                                int64_t lda, int64_t ldb, int64_t ldc)
 {
     if (groups < 2 || groups > 3) return (int)cudaErrorInvalidValue;
+    // one launch whatever the tile: the rule picks the shape, never a split
+    const TilePick t = choose_tile(TileProblem{ (int)M, (int)N, 0, 0, 0, groups, (int)((K + BLOCK_K - 1) / BLOCK_K), bt ? 1 : 0, false, false });
     CUtensorMap ma, mb[3];
     int a_swap = 0, b_swap = 0;
-    if (!make_map_rb(&ma, A, (uint64_t)K, (uint64_t)M, 1, (uint64_t)lda * 2, (uint64_t)(M * lda) * 2, BLOCK_K, BLOCK_M, &a_swap)) return (int)cudaErrorInvalidValue;
-    int64_t m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
+    if (!make_map_rb(&ma, A, (uint64_t)K, (uint64_t)M, 1, (uint64_t)lda * 2, (uint64_t)(M * lda) * 2, BLOCK_K, t.bm, &a_swap)) return (int)cudaErrorInvalidValue;
     for (int g = 0; g < groups; g++) {
         int sw = 0;
-        bool ok = bt ? make_map_rb(&mb[g], B[g], (uint64_t)K, (uint64_t)N, 1, (uint64_t)ldb * 2, (uint64_t)(N * ldb) * 2, BLOCK_K, BLOCK_N, &sw)
+        bool ok = bt ? make_map_rb(&mb[g], B[g], (uint64_t)K, (uint64_t)N, 1, (uint64_t)ldb * 2, (uint64_t)(N * ldb) * 2, BLOCK_K, t.bn, &sw)
                      : make_map_rb(&mb[g], B[g], (uint64_t)N, (uint64_t)K, 1, (uint64_t)ldb * 2, (uint64_t)(K * ldb) * 2, 64, BLOCK_K, &sw);
         if (!ok || (g > 0 && sw != b_swap)) return (int)cudaErrorInvalidValue;
         b_swap = sw;
     }
     TcParams p{};
     p.M = (int)M; p.N = (int)N; p.K = (int)K; p.batch = groups; p.groups = groups;
-    p.m_tiles = (int)m_tiles; p.n_tiles = (int)((N + BLOCK_N - 1) / BLOCK_N);
+    p.bm = t.bm; p.bn = t.bn;
+    p.m_tiles = (int)((M + t.bm - 1) / t.bm); p.n_tiles = (int)((N + t.bn - 1) / t.bn);
     p.b_kmajor = bt ? 1 : 0;
     p.a_swap = a_swap; p.b_swap = b_swap;
     p.taps = 1; p.kw = 1; p.bh = 0; p.bw = 0; p.tiles_x = 1;
@@ -807,7 +951,15 @@ int osb_tc_conv_launch(const void* x, const void* w, const void* bias, const voi
     if (gn_done) *gn_done = 0;
     if (gn_stats && (gn_groups < 1 || gn_groups > tcptx::GN_MAX_GROUPS || Cout % gn_groups || Cout % 8)) gn_stats = nullptr;
     const int gn_cpg = gn_stats ? (int)(Cout / gn_groups) : 0;
-    uint32_t bw = std::min<uint32_t>(128, next_pow2((uint32_t)Wo)), bh = 128 / bw;
+    const int k_blocks = kh * kw * (int)((Cin + BLOCK_K - 1) / BLOCK_K);
+    TileProblem q{ (int)(Ho * Wo), (int)Cout, (int)Ho, (int)Wo, 1, 1, k_blocks, 1, false, g_f32x != 0 };
+    const bool pair = !g_f32x && Cout % 8 == 0 && use_pair(problem_m_tiles(q, BLOCK_M), Cout);
+    // the split-K reduce paths move float4 / half4 vectors: ragged Cout (conv_out, 3 or 4 channels) and a residual that is not 8-byte
+    // aligned run unsplit
+    q.may_split = !pair && Cout % 4 == 0 && ((uintptr_t)residual & 7) == 0;
+    OsbWorkspace* wsp = nullptr;
+    const TilePick t = pair ? TilePick{ BLOCK_M, BLOCK_N, 1 } : choose_tile_ws(q, st, &wsp);
+    const uint32_t bw = (uint32_t)conv_box_w(t.bm, (int)Wo), bh = (uint32_t)t.bm / bw;
     CUtensorMap ma, mb;
     // A: NHWC input as (C, W, H); one box = bh rows x bw pixels x 64 channels, zero-filled outside the image.  With a
     // traversal stride s the box spans bw*s x bh*s input pixels and TMA delivers every s-th one.
@@ -815,37 +967,27 @@ int osb_tc_conv_launch(const void* x, const void* w, const void* bias, const voi
         return (int)cudaErrorInvalidValue;
     // B: OHWI weights = [Cout][kh*kw*Cin], K-major
     int64_t Ktot = (int64_t)kh * kw * Cin;
-    const int64_t m_tiles_ = ((Wo + bw - 1) / bw) * ((Ho + bh - 1) / bh);
-    const bool pair = !g_f32x && Cout % 8 == 0 && use_pair(m_tiles_, Cout);
-    if (!make_map(&mb, w, (uint64_t)Ktot, (uint64_t)Cout, 1, (uint64_t)Ktot * 2, (uint64_t)Ktot * Cout * 2, BLOCK_K, pair ? BLOCK_N / 2 : BLOCK_N, 1))
+    if (!make_map(&mb, w, (uint64_t)Ktot, (uint64_t)Cout, 1, (uint64_t)Ktot * 2, (uint64_t)Ktot * Cout * 2, BLOCK_K, pair ? BLOCK_N / 2 : t.bn, 1))
         return (int)cudaErrorInvalidValue;
     TcParams p{};
     p.M = (int)(Ho * Wo); p.N = (int)Cout; p.K = (int)Cin; p.batch = 1;
+    p.bm = t.bm; p.bn = t.bn;
     p.tiles_x = (int)((Wo + bw - 1) / bw);
     p.m_tiles = p.tiles_x * (int)((Ho + bh - 1) / bh);
-    p.n_tiles = (int)((Cout + BLOCK_N - 1) / BLOCK_N);
+    p.n_tiles = (int)((Cout + t.bn - 1) / t.bn);
     p.b_kmajor = 1;
     p.taps = kh * kw; p.kw = kw; p.pad_top = pad_top; p.pad_left = pad_left; p.Wo = (int)Wo; p.Ho = (int)Ho; p.bw = (int)bw; p.bh = (int)bh;
     p.k_blocks_per_tap = (int)((Cin + BLOCK_K - 1) / BLOCK_K);
     p.stride = stride;
     p.C = (__half*)y; p.bias = (const __half*)bias; p.residual = (const __half*)residual; p.stride_c = 0; p.ldc = Cout;
-    if (pair) {
-        p.split_k = 1;
-        p.bias2 = (const __half*)bias2;
-        if (gn_stats) { p.gn_stats = gn_stats; p.gn_cpg = gn_cpg; p.gn_groups = gn_groups; if (gn_done) *gn_done = 1; }
-        { static const int dbg = env_int("OSB_GN_DEBUG"); p.gn_debug = dbg; }
-        return launch(ma, mb, p, st, nullptr, nullptr, true);
-    }
-    // the split-K reduce paths move float4 / half4 vectors: ragged Cout (conv_out, 3 or 4 channels) and a residual that is not 8-byte
-    // aligned run unsplit
-    OsbWorkspace* wsp = nullptr;
-    p.split_k = (Cout % 4 == 0 && ((uintptr_t)residual & 7) == 0) ? choose_split(p.m_tiles * p.n_tiles, p.taps * p.k_blocks_per_tap, (size_t)Ho * Wo * Cout, st, &wsp) : 1;
+    p.split_k = t.split;
     p.ws = wsp ? wsp->splitk : nullptr;
     p.bias2 = (const __half*)bias2;
     // statistics: the tile epilogue (unsplit) or the reduce kernel (split-K; needs 4 consecutive columns inside one group)
-    const bool stats_ok = gn_stats && (p.split_k == 1 || gn_cpg % 4 == 0);     // tile epilogue (unsplit) or the reduce kernel
+    const bool stats_ok = gn_stats && (p.split_k == 1 || gn_cpg % 4 == 0);
     if (stats_ok) { p.gn_stats = gn_stats; p.gn_cpg = gn_cpg; p.gn_groups = gn_groups; if (gn_done) *gn_done = 1; }
     { static const int dbg = env_int("OSB_GN_DEBUG"); p.gn_debug = dbg; }
+    if (pair) return launch(ma, mb, p, st, nullptr, nullptr, true);
     if (g_f32x) {
         if (!f32x_params(p, wsp, st)) return (int)cudaErrorNotSupported;
     }

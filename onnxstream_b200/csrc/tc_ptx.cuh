@@ -170,65 +170,46 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 
 // Accumulator fragments of an m64nN wgmma: thread t of the warpgroup holds, for every 8-column block j, d[4j], d[4j+1] at row
 // 16 (t / 32) + (t % 32) / 4, columns 8j + 2 (t % 4) + {0, 1}, and d[4j+2], d[4j+3] at the row 8 below.
-template <int TRANS_B>
-__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d)
+// Shared-A wgmma (A and B from shared-memory descriptors), fp32 accumulators: m64nNk16 for the N the kernels use, in fp16 and bf16.
+// TC_R<n> is the asm list of n accumulator operands, TC_D<n> the matching "+f" operand list; the four operands after them are the A and B
+// descriptors, the scale-d flag and the B transpose immediate (their operand numbers are ODA, ODB, OSC, OTB).
+#define TC_R8(a, b, c, d, e, f, g, h) "%" #a ", %" #b ", %" #c ", %" #d ", %" #e ", %" #f ", %" #g ", %" #h
+#define TC_R16 TC_R8(0, 1, 2, 3, 4, 5, 6, 7) ", " TC_R8(8, 9, 10, 11, 12, 13, 14, 15)
+#define TC_R32 TC_R16 ", " TC_R8(16, 17, 18, 19, 20, 21, 22, 23) ", " TC_R8(24, 25, 26, 27, 28, 29, 30, 31)
+#define TC_R40 TC_R32 ", " TC_R8(32, 33, 34, 35, 36, 37, 38, 39)
+#define TC_R64 TC_R40 ", " TC_R8(40, 41, 42, 43, 44, 45, 46, 47) ", " TC_R8(48, 49, 50, 51, 52, 53, 54, 55) ", " TC_R8(56, 57, 58, 59, 60, 61, 62, 63)
+#define TC_R80 TC_R64 ", " TC_R8(64, 65, 66, 67, 68, 69, 70, 71) ", " TC_R8(72, 73, 74, 75, 76, 77, 78, 79)
+#define TC_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define TC_D16 TC_D8(0), TC_D8(8)
+#define TC_D32 TC_D16, TC_D8(16), TC_D8(24)
+#define TC_D40 TC_D32, TC_D8(32)
+#define TC_D64 TC_D40, TC_D8(40), TC_D8(48), TC_D8(56)
+#define TC_D80 TC_D64, TC_D8(64), TC_D8(72)
+#define TC_WGMMA_SS(N, TY, NAME, R, ODA, ODB, OSC, OTB, ...)                                                                                 \
+    template <int TRANS_B>                                                                                                              \
+    __device__ __forceinline__ void NAME(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d)                                 \
+    {                                                                                                                                   \
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " OSC ", 0;\n\t"                                                              \
+                     "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." TY "." TY " {" R "}, " ODA ", " ODB ", p, 1, 1, 0, " OTB ";\n\t}" \
+                     : __VA_ARGS__ : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));                                                     \
+    }
+#define TC_WGMMA_SS2(N, R, ODA, ODB, OSC, OTB, ...)                                      \
+    TC_WGMMA_SS(N, "f16", wgmma_m64n##N##k16_f16, R, ODA, ODB, OSC, OTB, __VA_ARGS__)   \
+    TC_WGMMA_SS(N, "bf16", wgmma_m64n##N##k16_bf16, R, ODA, ODB, OSC, OTB, __VA_ARGS__)
+TC_WGMMA_SS2(32, TC_R16, "%16", "%17", "%18", "%19", TC_D16)
+TC_WGMMA_SS2(64, TC_R32, "%32", "%33", "%34", "%35", TC_D32)
+TC_WGMMA_SS2(80, TC_R40, "%40", "%41", "%42", "%43", TC_D40)
+TC_WGMMA_SS2(128, TC_R64, "%64", "%65", "%66", "%67", TC_D64)
+TC_WGMMA_SS2(160, TC_R80, "%80", "%81", "%82", "%83", TC_D80)
+
+// m64nNk16 by N (the columns of one warpgroup's accumulator tile) and operand type
+template <int N, int TRANS_B, bool BF16>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d)
 {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, %67;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
-}
-template <int TRANS_B>
-__device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, %35;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
-}
-template <int TRANS_B>
-__device__ __forceinline__ void wgmma_m64n32k16_f16(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, %19;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
-}
-template <int TRANS_B>
-__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, %67;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
-}
-template <int TRANS_B>
-__device__ __forceinline__ void wgmma_m64n64k16_bf16(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, %35;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
-}
-template <int TRANS_B>
-__device__ __forceinline__ void wgmma_m64n32k16_bf16(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, %19;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(da), "l"(db), "r"(scale_d), "n"(TRANS_B));
+#define TC_CASE(n) if constexpr (N == n) { if constexpr (BF16) wgmma_m64n##n##k16_bf16<TRANS_B>(d, da, db, scale_d); else wgmma_m64n##n##k16_f16<TRANS_B>(d, da, db, scale_d); }
+    TC_CASE(32) TC_CASE(64) TC_CASE(80) TC_CASE(128) TC_CASE(160)
+#undef TC_CASE
+    static_assert(N == 32 || N == 64 || N == 80 || N == 128 || N == 160, "no wgmma wrapper for this N");
 }
 __device__ __forceinline__ void wgmma_m64n128k32_u8(int32_t (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d)
 {
