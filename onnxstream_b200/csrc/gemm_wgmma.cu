@@ -103,6 +103,18 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[WN / 2], uint64_t adesc,
     wgmma_commit();
 }
 
+// x[0], x[1] as a packed half2, columns outside the problem (ok0 / ok1 false) read as 0.  vec: the pair is 4-byte aligned, one load.
+// NC: through the read-only path (bias, bias2: never written by a launch; the residual may be C itself, so it takes plain loads).
+template <bool NC>
+__device__ __forceinline__ __half2 ld_pair(const __half* x, bool ok0, bool ok1, bool vec)
+{
+    const unsigned short* s = reinterpret_cast<const unsigned short*>(x);
+    uint32_t v;
+    if (ok1 && vec) v = NC ? __ldg(reinterpret_cast<const unsigned int*>(s)) : *reinterpret_cast<const unsigned int*>(s);
+    else v = (ok0 ? (uint32_t)(NC ? __ldg(s) : s[0]) : 0u) | (ok1 ? (uint32_t)(NC ? __ldg(s + 1) : s[1]) << 16 : 0u);
+    return *reinterpret_cast<__half2*>(&v);
+}
+
 // ---- the kernel -----------------------------------------------------------------------------------------------
 
 // BM x BN = the tile (TileCfg).  EXTRAS = the epilogue also adds `bias2` and gathers GroupNorm statistics.  A separate instantiation, so
@@ -231,6 +243,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         const bool partial = p.split_k > 1 || p.f32_out;
         const int r_lo = wrow + (warp & 3) * 16 + (lane >> 2);      // this thread's rows of the tile: r_lo and r_lo + 8
         const int cq = 2 * (lane & 3);                               // and its column pair inside every 8-column block
+        // the epilogue's column pairs load as one 4-byte word where the operand is aligned to it
+        const bool vec_bias = ((uintptr_t)p.bias & 3) == 0, vec_bias2 = ((uintptr_t)p.bias2 & 3) == 0;
+        const bool vec_res = ((uintptr_t)p.residual & 3) == 0 && ((p.ldc | p.stride_c) & 1) == 0;
         auto release = [&](int s) {
             if (PAIR) {
                 __syncwarp();
@@ -248,6 +263,35 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             const int n0 = nt * BN, c0 = n0 + wcol;      // tile and warpgroup column origins
             const int n_end = min(p.N, n0 + BN);
             const int kb_lo = sp * kb_per_split, kb_hi = min(kb_lo + kb_per_split, k_blocks_all);
+            long long out_row[2];   // row index into C (conv: output pixel index)
+            bool row_ok[2];
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int row_in_tile = r_lo + 8 * h;
+                if (p.bh > 0) {
+                    int y = (mt / p.tiles_x) * p.bh + row_in_tile / p.bw, x = (mt % p.tiles_x) * p.bw + row_in_tile % p.bw;
+                    row_ok[h] = y < p.Ho && x < p.Wo;
+                    out_row[h] = (long long)y * p.Wo + x;
+                } else {
+                    int m = mt * BM + row_in_tile;
+                    row_ok[h] = m < p.M;
+                    out_row[h] = m;
+                }
+            }
+            const long long off[2] = { (long long)b * p.stride_c + out_row[0] * p.ldc, (long long)b * p.stride_c + out_row[1] * p.ldc };
+            // The tile's residual rows are fetched into L2 while the main loop runs (a residual written several launches ago may have been
+            // evicted by the weights streaming through since), so the epilogue's loads do not wait on HBM.  The 4 lanes that share a row
+            // take one 128-byte line each of the warpgroup's (at most 320-byte) column span.
+            if (p.residual && !partial) {
+                const int span = (min(p.N, c0 + WN) - c0) * 2;
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const uintptr_t a0 = (uintptr_t)(p.residual + off[h] + c0), line = (a0 & ~(uintptr_t)127) + 128 * (lane & 3);
+                    if (row_ok[h] && span > 0 && line < a0 + span) {
+                        asm volatile("prefetch.global.L2 [%0];" ::"l"(line));
+                    }
+                }
+            }
 
             float acc[WN / 2];
 #pragma unroll
@@ -265,60 +309,63 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             release(prev);
 
             // ---- epilogue ----
-            long long out_row[2];   // row index into C (conv: output pixel index)
-            bool row_ok[2];
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int row_in_tile = r_lo + 8 * h;
-                if (p.bh > 0) {
-                    int y = (mt / p.tiles_x) * p.bh + row_in_tile / p.bw, x = (mt % p.tiles_x) * p.bw + row_in_tile % p.bw;
-                    row_ok[h] = y < p.Ho && x < p.Wo;
-                    out_row[h] = (long long)y * p.Wo + x;
-                } else {
-                    int m = mt * BM + row_in_tile;
-                    row_ok[h] = m < p.M;
-                    out_row[h] = m;
-                }
-            }
             __half* cbase = p.C;
             if (p.groups > 1) cbase = b == 0 ? p.C : (b == 1 ? p.C1 : p.C2);    // stride_c == 0 in a grouped launch
             const bool pair_ok = (p.N & 1) == 0 && (p.ldc & 1) == 0;           // two adjacent columns move as one 4- / 8-byte vector
+            // The addends of EG 8-column blocks are loaded before any of their stores: bias and residual may alias C for all the compiler
+            // knows, so it cannot move a block's loads above an earlier block's stores, and loads interleaved with the stores wait one by one.
+            constexpr int EG = 4;   // 2 and 8 measured no faster (DESIGN.md section 5)
 #pragma unroll
-            for (int j = 0; j < WN / 8; j++) {
-                if (c0 + 8 * j >= n_end) break;     // warp-uniform
-                const int n = c0 + 8 * j + cq;
-                const bool ok0 = n < n_end, ok1 = n + 1 < n_end;
-                float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;   // GroupNorm statistics of the two columns
-                float add0 = 0.f, add1 = 0.f;                   // per-column addends: bias (+ bias2)
-                if (!partial) {
-                    if (p.bias) { if (ok0) add0 += __half2float(p.bias[n]); if (ok1) add1 += __half2float(p.bias[n + 1]); }
-                }
+            for (int j0 = 0; j0 < WN / 8; j0 += EG) {
+                if (c0 + 8 * j0 >= n_end) break;    // warp-uniform
+                __half2 bias_v[EG], bias2_v[EG], res_v[EG][2];
 #pragma unroll
-                for (int h = 0; h < 2; h++) {
-                    if (!row_ok[h]) continue;
-                    float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-                    if (partial) {
-                        // split-K / fp32 output: raw fp32 partials, reduced (with bias / residual) by the reduce kernel
-                        float* wrow = p.ws + (((long long)sp * p.batch + b) * p.M + out_row[h]) * p.N;
-                        if (ok1 && pair_ok) *reinterpret_cast<float2*>(wrow + n) = make_float2(f0, f1);
-                        else { if (ok0) wrow[n] = f0; if (ok1) wrow[n + 1] = f1; }
-                        continue;
-                    }
-                    const long long off = (long long)b * p.stride_c + out_row[h] * p.ldc;
-                    f0 += add0; f1 += add1;
-                    if (p.residual) { if (ok0) f0 += __half2float(p.residual[off + n]); if (ok1) f1 += __half2float(p.residual[off + n + 1]); }
-                    if (EXTRAS && p.bias2) { if (ok0) f0 += __half2float(p.bias2[n]); if (ok1) f1 += __half2float(p.bias2[n + 1]); }
-                    const __half o0 = __float2half_rn(f0), o1 = __float2half_rn(f1);
-                    __half* crow = cbase + off;
-                    if (ok1 && pair_ok) *reinterpret_cast<__half2*>(crow + n) = __halves2half2(o0, o1);
-                    else { if (ok0) crow[n] = o0; if (ok1) crow[n + 1] = o1; }
-                    if (EXTRAS) {
-                        // the statistics see the values as they are stored
-                        const float g0 = ok0 ? __half2float(o0) : 0.f, g1 = ok1 ? __half2float(o1) : 0.f;
-                        s0 += g0; q0 = fmaf(g0, g0, q0); s1 += g1; q1 = fmaf(g1, g1, q1);
+                for (int jj = 0; jj < EG && j0 + jj < WN / 8; jj++) {
+                    const int n = c0 + 8 * (j0 + jj) + cq;
+                    const bool ok0 = n < n_end, ok1 = n + 1 < n_end;
+                    if (partial) continue;
+                    if (p.bias) bias_v[jj] = ld_pair<true>(p.bias + n, ok0, ok1, vec_bias);
+                    if (EXTRAS && p.bias2) bias2_v[jj] = ld_pair<true>(p.bias2 + n, ok0, ok1, vec_bias2);
+                    if (p.residual) {
+#pragma unroll
+                        for (int h = 0; h < 2; h++) res_v[jj][h] = ld_pair<false>(p.residual + off[h] + n, ok0 && row_ok[h], ok1 && row_ok[h], vec_res);
                     }
                 }
-                if (EXTRAS && p.gn_stats && !partial && !(p.gn_debug & 1)) gn_stats_pair(s0, s1, q0, q1, n, n_end, p.gn_cpg, gn_acc, lane);
+#pragma unroll
+                for (int jj = 0; jj < EG && j0 + jj < WN / 8; jj++) {
+                    const int j = j0 + jj;
+                    if (c0 + 8 * j >= n_end) break;     // warp-uniform
+                    const int n = c0 + 8 * j + cq;
+                    const bool ok0 = n < n_end, ok1 = n + 1 < n_end;
+                    float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;   // GroupNorm statistics of the two columns
+                    float add0 = 0.f, add1 = 0.f;                   // per-column addend: bias
+                    if (!partial && p.bias) { add0 += __low2float(bias_v[jj]); add1 += __high2float(bias_v[jj]); }
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        if (!row_ok[h]) continue;
+                        float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                        if (partial) {
+                            // split-K / fp32 output: raw fp32 partials, reduced (with bias / residual) by the reduce kernel
+                            float* wrow = p.ws + (((long long)sp * p.batch + b) * p.M + out_row[h]) * p.N;
+                            if (ok1 && pair_ok) *reinterpret_cast<float2*>(wrow + n) = make_float2(f0, f1);
+                            else { if (ok0) wrow[n] = f0; if (ok1) wrow[n + 1] = f1; }
+                            continue;
+                        }
+                        f0 += add0; f1 += add1;
+                        if (p.residual) { f0 += __low2float(res_v[jj][h]); f1 += __high2float(res_v[jj][h]); }
+                        if (EXTRAS && p.bias2) { f0 += __low2float(bias2_v[jj]); f1 += __high2float(bias2_v[jj]); }
+                        const __half o0 = __float2half_rn(f0), o1 = __float2half_rn(f1);
+                        __half* crow = cbase + off[h];
+                        if (ok1 && pair_ok) *reinterpret_cast<__half2*>(crow + n) = __halves2half2(o0, o1);
+                        else { if (ok0) crow[n] = o0; if (ok1) crow[n + 1] = o1; }
+                        if (EXTRAS) {
+                            // the statistics see the values as they are stored
+                            const float g0 = ok0 ? __half2float(o0) : 0.f, g1 = ok1 ? __half2float(o1) : 0.f;
+                            s0 += g0; q0 = fmaf(g0, g0, q0); s1 += g1; q1 = fmaf(g1, g1, q1);
+                        }
+                    }
+                    if (EXTRAS && p.gn_stats && !partial && !(p.gn_debug & 1)) gn_stats_pair(s0, s1, q0, q1, n, n_end, p.gn_cpg, gn_acc, lane);
+                }
             }
             if (EXTRAS && p.gn_stats && !partial && !(p.gn_debug & 2)) {
                 asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory");
