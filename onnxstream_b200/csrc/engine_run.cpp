@@ -123,6 +123,9 @@ struct Engine::Impl {
     // and zeroes the OTHER slot, which becomes current.  The whole ring is zeroed at the start of every run.
     DevPtr gn_ring;
     int gn_slot = 0;
+    // per slot: how many leading doubles the last statistics written into it cover (2 * its GroupNorm's groups).  The apply pass
+    // zeroes the other slot's first 2 * G doubles only; sums a GroupNorm with more groups left beyond them are zeroed separately.
+    int gn_slot_used[2] = { 0, 0 };
     long stats_want = -1;                 // set while a producer step runs: the GroupNorm step that wants its statistics
     int stats_groups = 0;
     long stats_ready_for = -1;            // GroupNorm step whose statistics sit in the current slot
@@ -1996,7 +1999,7 @@ void Engine::Impl::fused_groupnorm(const Step& s)
     // statistics the producer step left in the current ring slot; whoever does not consume them must zero the slot again
     const bool pre = stats_ready_for == (long)cur_step;
     stats_ready_for = -1;
-    auto drop_pre = [&] { if (pre) ck(cudaMemsetAsync(gn_slot_ptr(gn_slot), 0, 1024, st), "cudaMemsetAsync(gn slot)"); };
+    auto drop_pre = [&] { if (pre) { ck(cudaMemsetAsync(gn_slot_ptr(gn_slot), 0, 1024, st), "cudaMemsetAsync(gn slot)"); gn_slot_used[gn_slot] = 0; } };
     (void)in(i, 1); (void)in(i + 2, 1);  // the two shape constants (validated statically by the matcher)
     Tensor gs = in(i + 1, 1), gb = in(i + 1, 2), gamma = in(i + 3, 1), beta = in(i + 4, 1);
     int64_t C = x.shape[1], HW = x.numel() / C;
@@ -2020,8 +2023,13 @@ void Engine::Impl::fused_groupnorm(const Step& s)
         bool have = pre;
         if (!have) have = osb_channel_add_stats(x.data(), nullptr, nullptr, K(x.type), C, HW, G, gn_slot_ptr(gn_slot), st) == 0;
         if (have) {
+            gn_slot_used[gn_slot] = std::max(gn_slot_used[gn_slot], 2 * G);
             ck(osb_group_norm_apply(x.data(), y.mdata(), K(x.type), C, HW, G, gamma.data(), beta.data(), eps, s.count == 7 ? 1 : 0,
                                     gn_slot_ptr(gn_slot), gn_slot_ptr(gn_slot ^ 1), st), "osb_group_norm_apply");
+            int& other = gn_slot_used[gn_slot ^ 1];
+            if (other > 2 * G)
+                ck(cudaMemsetAsync(gn_slot_ptr(gn_slot ^ 1) + 2 * G, 0, (size_t)(other - 2 * G) * sizeof(double), st), "cudaMemsetAsync(gn slot tail)");
+            other = 0;
             gn_slot ^= 1;
             push(s.first + s.count - 1, 0, y);
             return;
@@ -2730,7 +2738,7 @@ void Engine::run()
         }
         if (!I.gn_ring) I.gn_ring = m_pool.alloc(2048);
         check_cuda(cudaMemsetAsync(I.gn_ring->ptr, 0, 2048, m_stream), "cudaMemsetAsync(gn ring)");    // both statistic slots zero: the invariant every producer relies on
-        I.gn_slot = 0; I.stats_ready_for = -1; I.stats_want = -1;
+        I.gn_slot = 0; I.gn_slot_used[0] = I.gn_slot_used[1] = 0; I.stats_ready_for = -1; I.stats_want = -1;
         I.mha_kv.clear();
         // side branch: steps off the critical path first, on their own stream and pool (see Impl::side_stream)
         bool hoist = !I.plan.is_side.empty() && resident_weights && !m_first_run && !has_i64_input && !ops_times_printf && !ops_printf && m_nranks == 1;

@@ -49,7 +49,7 @@ struct TileCfg {
     static constexpr int STAGES_FIT = RING_BYTES / (A_STAGE_BYTES + B_STAGE_BYTES);
     static constexpr int STAGES = STAGES_FIT < 16 ? STAGES_FIT : 16;      // 2 * STAGES mbarriers in the 256-byte barrier area
     static constexpr int WN = BM == 128 ? BN : BN / 2;                    // accumulator columns of one consumer warpgroup
-    static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * tcptx::GN_MAX_GROUPS * 4;
+    static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * tcptx::GN_MAX_GROUPS * 8;
     static_assert(BM == 64 || BM == 128, "BM");
     static_assert(BN % 16 == 0 && B_STAGE_BYTES % 1024 == 0, "every stage and every warpgroup's B rows start on a 1024-byte swizzle boundary");
 };
@@ -139,11 +139,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     uint64_t* bars = (uint64_t*)(smem + STAGES * (A_STAGE_BYTES + B_STAGE_BYTES));
     uint64_t* full = bars;                       // [STAGES]
     uint64_t* empty = bars + STAGES;             // [STAGES]
-    float* gn_acc = (float*)((uint8_t*)bars + 256);         // [2 * GN_MAX_GROUPS] per-CTA (sum, sum of squares) accumulators
+    double* gn_acc = (double*)((uint8_t*)bars + 256);       // [2 * GN_MAX_GROUPS] per-CTA (sum, sum of squares) accumulators
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    if (EXTRAS && p.gn_stats && threadIdx.x < 2 * GN_MAX_GROUPS) gn_acc[threadIdx.x] = 0.f;
+    if (EXTRAS && p.gn_stats && threadIdx.x < 2 * GN_MAX_GROUPS) gn_acc[threadIdx.x] = 0.0;
 
     if (warp == 0 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
@@ -279,6 +279,16 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 }
             }
             const long long off[2] = { (long long)b * p.stride_c + out_row[0] * p.ldc, (long long)b * p.stride_c + out_row[1] * p.ldc };
+            // GroupNorm statistics: the warp's valid rows (lanes 4r..4r+3 hold rows r (h = 0) and r + 8 (h = 1) of its 16), and the lane
+            // group + row half that holds the first of them -- each column's pivot is read from there (gn_stats_pair)
+            int gn_rows = 0, gn_src = 0, gn_h = 0;
+            if (EXTRAS && p.gn_stats) {
+                const unsigned b0 = __ballot_sync(0xffffffffu, row_ok[0]), b1 = __ballot_sync(0xffffffffu, row_ok[1]);
+                gn_rows = (__popc(b0) + __popc(b1)) >> 2;
+                gn_h = b0 ? 0 : 1;
+                gn_src = b0 ? __ffs(b0) - 1 : (b1 ? __ffs(b1) - 1 : 0);
+                gn_src = (gn_src & ~3) | (lane & 3);
+            }
             // The tile's residual rows are fetched into L2 while the main loop runs (a residual written several launches ago may have been
             // evicted by the weights streaming through since), so the epilogue's loads do not wait on HBM.  The 4 lanes that share a row
             // take one 128-byte line each of the warpgroup's (at most 320-byte) column span.
@@ -337,7 +347,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     if (c0 + 8 * j >= n_end) break;     // warp-uniform
                     const int n = c0 + 8 * j + cq;
                     const bool ok0 = n < n_end, ok1 = n + 1 < n_end;
-                    float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;   // GroupNorm statistics of the two columns
+                    float y0[2] = { 0.f, 0.f }, y1[2] = { 0.f, 0.f };   // the two columns as stored, for the GroupNorm statistics
                     float add0 = 0.f, add1 = 0.f;                   // per-column addend: bias
                     if (!partial && p.bias) { add0 += __low2float(bias_v[jj]); add1 += __high2float(bias_v[jj]); }
 #pragma unroll
@@ -360,11 +370,20 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         else { if (ok0) crow[n] = o0; if (ok1) crow[n + 1] = o1; }
                         if (EXTRAS) {
                             // the statistics see the values as they are stored
-                            const float g0 = ok0 ? __half2float(o0) : 0.f, g1 = ok1 ? __half2float(o1) : 0.f;
-                            s0 += g0; q0 = fmaf(g0, g0, q0); s1 += g1; q1 = fmaf(g1, g1, q1);
+                            y0[h] = ok0 ? __half2float(o0) : 0.f; y1[h] = ok1 ? __half2float(o1) : 0.f;
                         }
                     }
-                    if (EXTRAS && p.gn_stats && !partial && !(p.gn_debug & 1)) gn_stats_pair(s0, s1, q0, q1, n, n_end, p.gn_cpg, gn_acc, lane);
+                    if (EXTRAS && p.gn_stats && !partial && !(p.gn_debug & 1)) {
+                        const float p0 = __shfl_sync(0xffffffffu, gn_h ? y0[1] : y0[0], gn_src), p1 = __shfl_sync(0xffffffffu, gn_h ? y1[1] : y1[0], gn_src);
+                        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            if (!row_ok[h]) continue;
+                            const float d0 = y0[h] - p0, d1 = y1[h] - p1;
+                            s0 += d0; q0 = fmaf(d0, d0, q0); s1 += d1; q1 = fmaf(d1, d1, q1);
+                        }
+                        gn_stats_pair(s0, s1, q0, q1, p0, p1, gn_rows, n, n_end, p.gn_cpg, gn_acc, lane);
+                    }
                 }
             }
             if (EXTRAS && p.gn_stats && !partial && !(p.gn_debug & 2)) {
@@ -377,17 +396,34 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 }
 
 // split-K second pass: out[row][n] = fp16(sum_s ws[s][row][n] + bias[n] + bias2[n] + residual[row][n]); rows = batch * M.
-// Optionally gathers the GroupNorm statistics of the result (per-block shared accumulators -> global fp64).
+// Optionally gathers the GroupNorm statistics of the result as plain fp64 sums of y and y^2: per-block fp32 shared accumulators of
+// y - p around the group's pivot p (its first output, row 0, which every block computes alike), shifted back in fp64: each block adds s and
+// q + 2 p s, block 0 also n p and n p^2 for the n = rows * cpg elements of the group.
 __global__ void splitk_reduce_kernel(const float* __restrict__ ws, __half* __restrict__ out, const __half* __restrict__ bias, const __half* __restrict__ bias2,
                                      const __half* __restrict__ residual, long long rows, int N, int splits, double* __restrict__ gn_stats, int gn_cpg, int gn_groups)
 {
     osb_pdl_prologue();
     __shared__ float acc[2 * GN_MAX_GROUPS];
-    if (gn_stats) { if (threadIdx.x < 2 * GN_MAX_GROUPS) acc[threadIdx.x] = 0.f; __syncthreads(); }
+    __shared__ float piv[GN_MAX_GROUPS];
     // N % 4 == 0: one float4 of every split plane per thread, fully coalesced
     const long long total4 = rows * N / 4;
     const long long plane4 = total4;
     const float4* w4 = reinterpret_cast<const float4*>(ws);
+    if (gn_stats) {
+        if (threadIdx.x < 2 * GN_MAX_GROUPS) acc[threadIdx.x] = 0.f;
+        if (threadIdx.x < gn_groups) {
+            // group g's pivot: the output at row 0, column g * cpg, as the loop below computes and rounds it
+            const int n = threadIdx.x * gn_cpg;
+            float v = ws[n];
+#pragma unroll 8
+            for (int s = 1; s < splits; s++) v += __ldg(ws + (long long)s * rows * N + n);    // independent loads: few round trips
+            if (bias) v += __half2float(bias[n]);
+            if (bias2) v += __half2float(bias2[n]);
+            if (residual) v += __half2float(residual[n]);
+            piv[threadIdx.x] = __half2float(__float2half_rn(v));
+        }
+        __syncthreads();
+    }
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4; i += (long long)gridDim.x * blockDim.x) {
         float4 a = w4[i];
         for (int s = 1; s < splits; s++) { float4 t = w4[(long long)s * plane4 + i]; a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w; }
@@ -404,15 +440,21 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, __half* __res
         store_vec<__half, 4>(out + e, o);
         if (gn_stats) {
             // the 4 columns of a thread lie in one group when cpg % 4 == 0 (host guarantees it)
-            float x0 = __half2float(o.v[0]), x1 = __half2float(o.v[1]), x2 = __half2float(o.v[2]), x3 = __half2float(o.v[3]);
             const int g = n / gn_cpg;
+            const float pg = piv[g];
+            float x0 = __half2float(o.v[0]) - pg, x1 = __half2float(o.v[1]) - pg, x2 = __half2float(o.v[2]) - pg, x3 = __half2float(o.v[3]) - pg;
             atomicAdd(&acc[2 * g], (x0 + x1) + (x2 + x3));
             atomicAdd(&acc[2 * g + 1], fmaf(x0, x0, x1 * x1) + fmaf(x2, x2, x3 * x3));
         }
     }
     if (gn_stats) {
         __syncthreads();
-        if (threadIdx.x < 2 * gn_groups) { float v = acc[threadIdx.x]; if (v != 0.f) atomicAdd(&gn_stats[threadIdx.x], (double)v); }
+        if (threadIdx.x < gn_groups) {
+            const int g = threadIdx.x;
+            const double s = acc[2 * g], q = acc[2 * g + 1], pg = piv[g], n = blockIdx.x == 0 ? (double)rows * gn_cpg : 0.0;
+            atomicAdd(&gn_stats[2 * g], s + n * pg);
+            atomicAdd(&gn_stats[2 * g + 1], q + (2.0 * pg) * s + n * pg * pg);
+        }
     }
 }
 

@@ -522,19 +522,30 @@ __global__ void gn_stats_nhwc_kernel(const T* __restrict__ x, double* __restrict
     for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) atomicAdd(&stats[i], (double)sm[i]);
 }
 
+// y's value at pixel 0, channel c (y = x, or x + addv[c] rounded to T): the pivot of the group that starts at channel c, which
+// every CTA computes alike
+template <typename T>
+__device__ __forceinline__ float gn_first_y(const T* __restrict__ x, const T* __restrict__ addv, int c)
+{
+    const float v = to_float(x[c]);
+    return addv ? to_float(from_float<T>(v + to_float(addv[c]))) : v;
+}
+
 // NHWC statistics, vectorised: a thread owns 8 consecutive channels (one 16-byte load per pixel) and walks down the
-// CTA's pixel strip; 256/(C/8) pixels are in flight per iteration.  Per-channel partials are folded into the 2*G group
-// bins with shared-memory atomics, then one double atomic per bin and CTA.
+// CTA's pixel strip; 256/(C/8) pixels are in flight per iteration.  Per-channel fp32 partials of y - p (p: the group's pivot,
+// gn_first_y) go to shared memory, are folded per group in fp64, then one double atomic per bin and CTA.
 template <typename T, int VEC>
 __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __restrict__ stats, int C, int64_t HW, int groups, int64_t pix_per_cta,
                                          const T* __restrict__ addv = nullptr, T* __restrict__ y = nullptr, int pivot = 0)
 {
     // addv / y != null: y = x + addv[c] (the per-channel time-embedding add of a resnet) is written on the way and the statistics
-    // are those of y -- the producer side of a GroupNorm whose apply pass is gn_apply_pre_kernel.  pivot != 0: sums of x - p around
-    // the group pivot (osb_group_norm's layout, see gn_mean_var); else plain sums, which gn_apply_pre_kernel reads
+    // are those of y -- the producer side of a GroupNorm whose apply pass is gn_apply_pre_kernel.  pivot != 0: the sums of y - p
+    // go out as they are (osb_group_norm's layout, see gn_mean_var); else they are shifted back to plain sums of y and y^2, which
+    // gn_apply_pre_kernel reads: S += s + n p, Q += q + 2 p s + n p^2 in fp64 with n the CTA's element count of the group.  Plain fp32
+    // sums of y and y^2 would cancel in E[y^2] - mean^2 when the mean is large against the spread.
     osb_pdl_prologue();
-    extern __shared__ float sm[];  // 2 * groups
-    for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) sm[i] = 0.f;
+    extern __shared__ float sm[];  // the group pivots (groups of the 2 * groups floats), then the per-row partials
+    for (int g = threadIdx.x; g < groups; g += blockDim.x) sm[g] = gn_first_y(x, addv, g * (C / groups));
     __syncthreads();
     const int tpp = C / VEC;                        // threads per pixel
     const int rows = blockDim.x / tpp;              // pixels in flight
@@ -544,7 +555,7 @@ __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __rest
     if (pr < rows) {
         float s[VEC], q[VEC], a[VEC], pv[VEC];
 #pragma unroll
-        for (int k = 0; k < VEC; k++) { s[k] = 0.f; q[k] = 0.f; a[k] = 0.f; pv[k] = pivot ? to_float(x[(cv * VEC + k) / cpg * cpg]) : 0.f; }
+        for (int k = 0; k < VEC; k++) { s[k] = 0.f; q[k] = 0.f; a[k] = 0.f; pv[k] = sm[(cv * VEC + k) / cpg]; }
         if (addv) {
             Vec<T, VEC> av = load_vec<T, VEC>(addv + cv * VEC);
 #pragma unroll
@@ -575,16 +586,26 @@ __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __rest
     }
     __syncthreads();
     {
-        // thread t < 2 * groups: group t / 2, statistic t % 2 -- sums its cpg channels over the pixel rows of the CTA
+        // bin b = 2 g + which (which: 0 = sum, 1 = sum of squares) is summed in fp64 by tpb adjacent threads, each taking every tpb-th
+        // of its rows x cpg partials, then combined by shuffle; bins 2 g and 2 g + 1 sit in one warp for the shift back
         const float* part = sm + 2 * groups;
-        for (int t = threadIdx.x; t < 2 * groups; t += blockDim.x) {
-            const int g = t >> 1, which = t & 1;
-            float acc = 0.f;
-            for (int r = 0; r < rows; r++) {
-                const float* rowp = part + (r * 2 + which) * C + g * cpg;
-                for (int c = 0; c < cpg; c++) acc += rowp[c];
+        int tpb = 16;
+        while (tpb > 1 && tpb * 2 * groups > (int)blockDim.x) tpb >>= 1;
+        const int b = threadIdx.x / tpb, sub = threadIdx.x % tpb, g = b >> 1, which = b & 1;
+        double v = 0.0;
+        if (b < 2 * groups)
+            for (int r = 0; r < rows; r++)
+                for (int c = sub; c < cpg; c += tpb) v += part[(r * 2 + which) * C + g * cpg + c];
+#pragma unroll
+        for (int off = 1; off < 16; off <<= 1)
+            if (off < tpb) v += __shfl_xor_sync(0xffffffffu, v, off);
+        const double s_of_group = __shfl_xor_sync(0xffffffffu, v, which ? tpb : 0);   // the group's sum, in both bins' threads
+        if (b < 2 * groups && sub == 0) {
+            if (!pivot) {
+                const double pg = sm[g], n = (double)(p1 - p0) * cpg;
+                v += which ? (2.0 * pg) * s_of_group + n * pg * pg : n * pg;
             }
-            atomicAdd(&stats[t], (double)acc);
+            atomicAdd(&stats[b], v);
         }
     }
 }
@@ -599,8 +620,11 @@ gn_fused_nhwc_kernel(const T* __restrict__ x, T* __restrict__ y, double* __restr
                      int C, int64_t HW, int groups, int64_t pix_per_cta, const T* __restrict__ gamma, const T* __restrict__ beta, float eps, int silu)
 {
     osb_pdl_prologue();
-    extern __shared__ float sm[];  // 2 * groups partials, then 2 * groups (mean, rstd)
-    for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) sm[i] = 0.f;
+    // 2 * groups fp64 partials, then (as floats) 2 * groups (mean, rstd).  The per-thread fp32 partials are combined in fp64, as the
+    // producers of gn_apply_pre_kernel's statistics do, so that both GroupNorm paths derive the same mean and rstd from the same input.
+    extern __shared__ double smd[];
+    float* sm = reinterpret_cast<float*>(smd);
+    for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) smd[i] = 0.0;
     __syncthreads();
     const int tpp = C / VEC;
     const int rows = blockDim.x / tpp;
@@ -619,18 +643,19 @@ gn_fused_nhwc_kernel(const T* __restrict__ x, T* __restrict__ y, double* __restr
         // combine the channels of this vector that fall into the same group in registers first: 2 (not 2 * VEC) shared atomics
         // per group touched -- the contended shared atomics were the longest phase of the kernel
         int g_cur = (cv * VEC) / cpg;
-        float gs = 0.f, gq = 0.f;
+        double gs = 0.0, gq = 0.0;
 #pragma unroll
         for (int k = 0; k < VEC; k++) {
             int g = (cv * VEC + k) / cpg;
-            if (g != g_cur) { atomicAdd(&sm[2 * g_cur], gs); atomicAdd(&sm[2 * g_cur + 1], gq); g_cur = g; gs = 0.f; gq = 0.f; }
+            if (g != g_cur) { atomicAdd(&smd[2 * g_cur], gs); atomicAdd(&smd[2 * g_cur + 1], gq); g_cur = g; gs = 0.0; gq = 0.0; }
             gs += s[k]; gq += q[k];
         }
-        atomicAdd(&sm[2 * g_cur], gs);
-        atomicAdd(&sm[2 * g_cur + 1], gq);
+        atomicAdd(&smd[2 * g_cur], gs);
+        atomicAdd(&smd[2 * g_cur + 1], gq);
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) atomicAdd(&stats[i], (double)sm[i]);
+    for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) atomicAdd(&stats[i], smd[i]);
+    __syncthreads();      // every partial is read before sm (the same memory) takes the (mean, rstd) floats
     // ---- grid rendezvous ----
     __threadfence();
     __syncthreads();
@@ -661,14 +686,14 @@ gn_fused_nhwc_kernel(const T* __restrict__ x, T* __restrict__ y, double* __restr
 #pragma unroll
         for (int k = 0; k < VEC; k++) {
             int c = cv * VEC + k, g = c / cpg;
-            gm[k] = gamma ? to_float(gamma[c]) : 1.f; bt[k] = beta ? to_float(beta[c]) : 0.f; mu[k] = sm[2 * g]; rs[k] = sm[2 * g + 1];
+            gm[k] = gamma ? to_float(gamma[c]) : 1.f; bt[k] = beta ? to_float(beta[c]) : 0.f; mu[k] = sm[2 * g]; rs[k] = sm[2 * g + 1] * gm[k];
         }
         for (int64_t p = p0 + pr; p < p1; p += rows) {
             Vec<T, VEC> v = load_vec<T, VEC>(x + p * C + cv * VEC);
 #pragma unroll
             for (int k = 0; k < VEC; k++) {
-                float o = (to_float(v.v[k]) - mu[k]) * rs[k] * gm[k] + bt[k];
-                if (silu) o = o / (1.f + __expf(-o));
+                float o = fmaf(to_float(v.v[k]) - mu[k], rs[k], bt[k]);      // rs: rstd * gamma, as gn_apply_pre_kernel's scale
+                if (silu) o = __fdividef(o, 1.f + __expf(-o));
                 v.v[k] = from_float<T>(o);
             }
             store_vec<T, VEC>(y + p * C + cv * VEC, v);
@@ -734,16 +759,19 @@ __global__ void gn_apply_kernel(const T* __restrict__ x, T* __restrict__ y, cons
 
 
 // GroupNorm(+SiLU) apply pass for statistics gathered by the producing conv's epilogue (osb_conv2d_ex): one streaming pass, no grid
-// rendezvous.  Each CTA folds (mean, rstd, gamma, beta) into a per-channel (scale, shift) table in shared memory, then y = x * scale[c] +
-// shift[c] over its strip of NHWC pixels with 16-byte vectors.  CTA 0 zeroes `clear_stats` -- the buffer the NEXT statistics producer
-// in stream order accumulates into (its previous reader finished before this kernel started).
+// rendezvous.  Each CTA lays out per-channel mean, scale = rstd * gamma and beta tables in shared memory, then y = (x - mean) * scale +
+// beta (+ SiLU) over its strip of NHWC pixels with 16-byte vectors, a thread's VEC channels read from each table as 16-byte words.  This
+// is gn_fused_nhwc_kernel's arithmetic, so a GroupNorm computes the same from the same statistics on either path.  The subtraction comes
+// first: x * scale + (beta - mean * scale) would round mean * scale at the scale of the mean, several ulps of the mean times rstd when the
+// mean is large against the spread.  CTA 0 zeroes `clear_stats` -- the buffer the NEXT statistics producer in stream order accumulates
+// into (its previous reader finished before this kernel started).
 template <typename T, int VEC>
 __global__ void gn_apply_pre_kernel(const T* __restrict__ x, T* __restrict__ y, const double* __restrict__ stats, double* __restrict__ clear_stats,
                                     int C, int64_t HW, int groups, const T* __restrict__ gamma, const T* __restrict__ beta, float eps, int silu)
 {
     osb_pdl_prologue();
-    extern __shared__ float tab[];          // [2 * C]: scale, shift
-    float* scale = tab; float* shift = tab + C;
+    extern __shared__ float4 tab4[];        // [3 * C] floats: mean, scale, beta
+    float* mu = reinterpret_cast<float*>(tab4); float* scale = mu + C; float* shift = mu + 2 * C;
     const int cpg = C / groups;
     const double inv_n = 1.0 / ((double)cpg * (double)HW);
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -752,8 +780,7 @@ __global__ void gn_apply_pre_kernel(const T* __restrict__ x, T* __restrict__ y, 
         const double var = stats[2 * g + 1] * inv_n - mean * mean;
         const float rstd = rsqrtf(fmaxf((float)var, 0.f) + eps);
         const float ga = gamma ? to_float(gamma[c]) : 1.f, be = beta ? to_float(beta[c]) : 0.f;
-        scale[c] = rstd * ga;
-        shift[c] = be - (float)mean * rstd * ga;
+        mu[c] = (float)mean; scale[c] = rstd * ga; shift[c] = be;
     }
     if (blockIdx.x == 0 && clear_stats) for (int t = threadIdx.x; t < 2 * groups; t += blockDim.x) clear_stats[t] = 0.0;
     __syncthreads();
@@ -770,9 +797,16 @@ __global__ void gn_apply_pre_kernel(const T* __restrict__ x, T* __restrict__ y, 
             const int64_t i = i0 + u * stride;
             if (i >= nvec) break;
             const int c0 = (int)(i % vpp) * VEC;
+            float tm[VEC], ts[VEC], tb[VEC];
+#pragma unroll
+            for (int k = 0; k < VEC; k += 4) {
+                *reinterpret_cast<float4*>(tm + k) = *reinterpret_cast<const float4*>(mu + c0 + k);
+                *reinterpret_cast<float4*>(ts + k) = *reinterpret_cast<const float4*>(scale + c0 + k);
+                *reinterpret_cast<float4*>(tb + k) = *reinterpret_cast<const float4*>(shift + c0 + k);
+            }
 #pragma unroll
             for (int k = 0; k < VEC; k++) {
-                float o = fmaf(to_float(v[u].v[k]), scale[c0 + k], shift[c0 + k]);
+                float o = fmaf(to_float(v[u].v[k]) - tm[k], ts[k], tb[k]);
                 if (silu) o = __fdividef(o, 1.f + __expf(-o));
                 v[u].v[k] = from_float<T>(o);
             }
@@ -1343,7 +1377,7 @@ int osb_group_norm(const void* x, void* y, int dtype, int nhwc, int64_t C, int64
             // one CTA per SM by default (every CTA must be co-resident for the rendezvous; fewer CTAs = fewer same-address atomics)
             static const int cta_cap = [] { const char* e = getenv("OSB_GN_CTAS"); int v = e ? atoi(e) : 0; return v > 0 ? v : OSB_SMS; }();
             int threads = C / vec <= 256 ? 256 : 512;
-            size_t smem = sizeof(float) * 2 * groups;
+            size_t smem = sizeof(double) * 2 * groups;
             // co-residency bound from the device itself (SM count x resident CTAs of THIS kernel at this block size), and a cooperative
             // launch so the driver gang-schedules the grid: with SMs held by other work the launch waits (or fails) instead of spinning
             int dev = 0, sms = 0, occ = 0;
@@ -1420,7 +1454,7 @@ int osb_group_norm_apply(const void* x, void* y, int dtype, int64_t C, int64_t H
     const int vec = dtype == OSB_F16 ? 8 : 4;
     if (groups < 1 || C % groups || C % vec || C > 4096 || !aligned16(x) || !aligned16(y)) return (int)cudaErrorInvalidValue;
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t smem = sizeof(float) * 2 * (size_t)C;
+    const size_t smem = sizeof(float) * 3 * (size_t)C;      // <= 48 KB (C <= 4096)
     const int64_t nvec = HW * (C / vec);
     // every CTA pays the table set-up (C channels, a few hundred cycles); 4 vectors per thread per pass, up to 4 CTAs per SM
     const int grid = (int)max<int64_t>(1, min<int64_t>((nvec + 256 * 4 - 1) / (256 * 4), OSB_SMS * 4));

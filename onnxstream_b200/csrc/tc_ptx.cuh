@@ -245,33 +245,58 @@ __device__ __forceinline__ void wgmma_m64n64k16_bf16_rs(float (&d)[32], const ui
 // The consumer GroupNorm needs sum(x) and sum(x^2) per group of `cpg` consecutive channels over ALL rows (pixels).  A thread holds two
 // adjacent columns of two rows per 8-column block (the accumulator fragment above): the 8 lanes that share those columns sum their rows by
 // shuffle, and lanes 0..3 add the column totals to the CTA's per-group shared accumulators.  After the tile the accumulators are flushed to
-// the global fp64 statistics (the reference accumulates in double) -- fp32 only ever sums <= 128 rows x cpg values.
+// the global fp64 statistics (the reference accumulates in double).  Plain fp32 sums of y and y^2 would cancel in E[y^2] - mean^2 when
+// the mean is large against the spread, so a column's fp32 warp partial is of y - p, p = that column's value in the warp's first valid
+// row, and is shifted back in fp64 (S += s + c p, Q += q + 2 p s + c p^2, c = the warp's valid rows) into fp64 CTA accumulators.
 constexpr int GN_MAX_GROUPS = 64;
 
-// v0 / v1: this thread's two columns (n, n + 1), each summed over its two rows, values already rounded as they are stored (rows outside
-// the problem passed as zeros); q0 / q1 the same for the squares
-__device__ __forceinline__ void gn_stats_pair(float v0, float v1, float q0, float q1, int n, int n_end, int cpg, float* cta_stats, int lane)
+// fp64 add into shared memory (a CAS loop in SASS; the explicit state space keeps the compiler from adding a global-memory path)
+__device__ __forceinline__ void shared_add_f64(double* p, double v)
+{
+    asm volatile("red.shared.add.f64 [%0], %1;" ::"r"(smem_u32(p)), "d"(v) : "memory");
+}
+
+// v0 / v1: this thread's two columns (n, n + 1), each summed over its valid rows as y - p0 / y - p1 with y rounded as it is stored
+// (columns outside the problem passed as zeros); q0 / q1 the same for the squares; c: the warp's valid rows.  Lanes 0..3 (the 8 columns
+// of the block) combine their fp64 sums by group before the shared adds: one per group the block touches, not one per lane.
+__device__ __forceinline__ void gn_stats_pair(float v0, float v1, float q0, float q1, float p0, float p1, int c, int n, int n_end, int cpg,
+                                              double* cta_stats, int lane)
 {
 #pragma unroll
     for (int off = 4; off < 32; off <<= 1) {
         v0 += __shfl_xor_sync(0xffffffffu, v0, off); v1 += __shfl_xor_sync(0xffffffffu, v1, off);
         q0 += __shfl_xor_sync(0xffffffffu, q0, off); q1 += __shfl_xor_sync(0xffffffffu, q1, off);
     }
-    if (lane < 4 && n < n_end) {
-        const int g0 = n / cpg;
-        if (n + 1 < n_end && (n + 1) / cpg == g0) { v0 += v1; q0 += q1; }
-        else if (n + 1 < n_end) { atomicAdd(&cta_stats[2 * (g0 + 1)], v1); atomicAdd(&cta_stats[2 * (g0 + 1) + 1], q1); }
-        atomicAdd(&cta_stats[2 * g0], v0);
-        atomicAdd(&cta_stats[2 * g0 + 1], q0);
+    const double dc = (double)c, d0 = p0, d1 = p1;
+    const bool ok0 = n < n_end && c > 0, ok1 = n + 1 < n_end && c > 0;
+    const int g0 = n / cpg;
+    double s = ok0 ? (double)v0 + dc * d0 : 0.0, r = ok0 ? (double)q0 + (2.0 * d0) * v0 + dc * d0 * d0 : 0.0;
+    if (ok1) {
+        const double s1 = (double)v1 + dc * d1, r1 = (double)q1 + (2.0 * d1) * v1 + dc * d1 * d1;
+        if ((n + 1) / cpg == g0) { s += s1; r += r1; }
+        else if (lane < 4) { shared_add_f64(&cta_stats[2 * (g0 + 1)], s1); shared_add_f64(&cta_stats[2 * (g0 + 1) + 1], r1); }
     }
+    // segmented sum over lanes 0..3 by group (groups are contiguous, so lane l's group <= lane l + 1's): lane 2k takes lane 2k + 1,
+    // then lane 0 takes lane 2; a lane whose sums were taken adds nothing itself
+    const int g = ok0 ? g0 : -1;
+    bool taken = false;
+#pragma unroll
+    for (int off = 1; off < 4; off <<= 1) {
+        const double so = __shfl_down_sync(0xffffffffu, s, off), ro = __shfl_down_sync(0xffffffffu, r, off);
+        const int go = __shfl_down_sync(0xffffffffu, g, off);
+        const int gu = __shfl_up_sync(0xffffffffu, g, off);
+        if ((lane & (2 * off - 1)) == 0 && go == g && g >= 0) { s += so; r += ro; }
+        if ((lane & (2 * off - 1)) == off && gu == g) taken = true;
+    }
+    if (lane < 4 && g >= 0 && !taken) { shared_add_f64(&cta_stats[2 * g], s); shared_add_f64(&cta_stats[2 * g + 1], r); }
 }
 
 // after a tile: thread t of the epilogue group moves accumulator t to the global fp64 statistics and re-arms it
-__device__ __forceinline__ void gn_stats_flush(float* cta_stats, double* gstats, int groups, int t)
+__device__ __forceinline__ void gn_stats_flush(double* cta_stats, double* gstats, int groups, int t)
 {
     if (t < 2 * groups) {
-        const float v = atomicExch(&cta_stats[t], 0.f);
-        if (v != 0.f) atomicAdd(&gstats[t], (double)v);
+        const double v = __longlong_as_double((long long)atomicExch(reinterpret_cast<unsigned long long*>(&cta_stats[t]), 0ull));
+        if (v != 0.0) atomicAdd(&gstats[t], v);
     }
 }
 

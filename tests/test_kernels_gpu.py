@@ -351,6 +351,8 @@ def test_conv_epilogue_gn_stats_and_bias2(K, case):
     want = torch.stack([yd.sum(dim=(0, 2)), (yd * yd).sum(dim=(0, 2))], dim=1).reshape(-1)
     err = (stats - want).abs() / (torch.stack([yd.abs().sum(dim=(0, 2)), (yd * yd).sum(dim=(0, 2))], dim=1).reshape(-1) + 1e-9)
     assert float(err.max()) <= 2e-5, f"statistics off by {float(err.max()):.3g} (relative to sum|y| / sum y^2)"
+    from test_node_kernels_gpu import _check_gn_slot, _gn_ref, _gn_tol
+    _check_gn_slot(stats, y.double().cpu().numpy(), Ho * Wo, Cout, G, f"conv_ex {case}")
     # apply pass: GroupNorm + SiLU from those statistics; the `clear` buffer is zeroed on the way
     gamma = (1 + 0.1 * torch.randn(Cout, device="cuda", generator=g)).half(); beta = (0.1 * torch.randn(Cout, device="cuda", generator=g)).half()
     out = torch.empty_like(y); clear = torch.ones(2 * G, device="cuda", dtype=torch.float64)
@@ -360,6 +362,9 @@ def test_conv_epilogue_gn_stats_and_bias2(K, case):
     gn = ((yd - mean) / torch.sqrt(var + 1e-5)).reshape(Ho, Wo, Cout) * gamma.double() + beta.double()
     gn = gn * torch.sigmoid(gn)
     assert float((out.double() - gn).abs().max()) <= 2e-3 * max(1.0, float(gn.abs().max()))
+    ref, mean, rg = _gn_ref(y.double().cpu().numpy().reshape(-1), 1, Cout, Ho * Wo, G, gamma.double().cpu().numpy(), beta.double().cpu().numpy(), 1)
+    tol = _gn_tol(ref, mean, rg, F16)
+    assert (np.abs(out.double().cpu().numpy().reshape(-1) - ref) <= tol).all(), "GroupNorm from the epilogue statistics outside _gn_tol"
     assert float(clear.abs().max()) == 0.0
 
 
@@ -379,6 +384,8 @@ def test_channel_add_stats(K):
         want = torch.stack([yd.sum(dim=(0, 2)), (yd * yd).sum(dim=(0, 2))], dim=1).reshape(-1)
         scale = torch.stack([yd.abs().sum(dim=(0, 2)), (yd * yd).sum(dim=(0, 2))], dim=1).reshape(-1)
         assert float(((stats - want).abs() / scale).max()) <= 2e-5
+        from test_node_kernels_gpu import _check_gn_slot
+        _check_gn_slot(stats, y.double().cpu().numpy(), HW, C, G, f"channel_add_stats HW {HW} C {C} G {G}")
 
 
 def test_qu8_gemm_and_conv_bit_exact(K):

@@ -372,52 +372,143 @@ def test_group_norm_offset_mean(K, path, nhwc, C, HW, G, yoff, launches, dtype, 
         _assert_within(out, ref, _gn_tol(ref, mean, rg, dtype), f"{path} m = {m}, launch {i + 1}")
 
 
-@pytest.mark.xfail(reason="osb_channel_add_stats hands gn_apply_pre_kernel plain fp32 per-CTA sums of y and y^2, which cancel in "
-                          "E[y^2] - mean^2 when the mean is large against the spread", strict=False)
-def test_channel_add_stats_offset_mean(K):
-    """osb_channel_add_stats (statistics of y = x + t[c] in the vector statistics kernel) + osb_group_norm_apply at x = 1024 + N(0, 1):
-    GroupNorm(+SiLU) of the stored y against fp64.  Bar: _gn_tol (fp16)."""
+# ---- producer statistics (plain fp64 sums of y and y^2 in a two-slot ring) -> osb_group_norm_apply, at large means ----------------
+
+STATS_M = [0.0, 16.0, 64.0, 256.0, 1024.0]         # mean / spread of the GroupNorm input
+
+
+def _check_gn_slot(stats, yd, HW, C, G, what):
+    """The mean and variance osb_group_norm_apply derives from a statistics slot (plain sums S, Q: mean = S/n, var = Q/n - mean^2, in fp64)
+    against the fp64 two-pass statistics of the stored y ([HW, C]).  Bar, relative to the variance (not to sum y^2, which is larger by
+    1 + mean^2/var): the producers sum y - p in fp32 (p: one stored y of the group, so sum (y - p)^2 is a small multiple of n var) over
+    chains of at most a few hundred values, then shift back in fp64 -- |d var| <= 2^-14 var; and the fp64 sums themselves carry a few
+    ulps at the mean's scale -- + 2^-48 mean^2.  The mean: |d mean| <= 2^-14 sqrt(var) + 2^-48 |mean|.  Returns the worst error / bar."""
+    st = stats.cpu().numpy().astype(np.float64).reshape(-1)[:2 * G].reshape(G, 2)
+    grp = yd.reshape(HW, G, C // G).transpose(1, 0, 2).reshape(G, -1)
+    n = grp.shape[1]
+    mean = grp.mean(1)
+    var = ((grp - mean[:, None]) ** 2).mean(1)
+    gm = st[:, 0] / n
+    gv = st[:, 1] / n - gm * gm
+    bar_m = 2.0 ** -14 * np.sqrt(var) + 2.0 ** -48 * np.abs(mean)
+    bar_v = 2.0 ** -14 * var + 2.0 ** -48 * mean * mean
+    rm, rv = np.abs(gm - mean) / bar_m, np.abs(gv - var) / bar_v
+    worst = float(max(rm.max(), rv.max()))
+    print(f"[bar] gn-slot {what}: mean {float(rm.max()):.3g}, var {float(rv.max()):.3g} of the bar")
+    assert rm.max() <= 1.0 and rv.max() <= 1.0, (f"{what}: slot statistics off: mean err/bar {float(rm.max()):.3g} (group {int(rm.argmax())}), "
+                                                 f"var err/bar {float(rv.max()):.3g} (group {int(rv.argmax())}, var {var[rv.argmax()]:.4g}, "
+                                                 f"got {gv[rv.argmax()]:.6g}, mean {mean[rv.argmax()]:.4g})")
+    return worst
+
+
+def _check_gn_apply_from_slot(K, y, stats, dtype, HW, C, G, seed, what):
+    """osb_group_norm_apply (GroupNorm + SiLU) on the slot against fp64 GroupNorm of the stored y; the other slot must come back zeroed.
+    Bar: _gn_tol."""
     import torch
-    HW, C, G = 4096, 320, 32
-    rng = np.random.default_rng(5)
-    x = torch.from_numpy((1024.0 + rng.standard_normal((HW, C))).astype(np.float16)).cuda()
-    t = torch.from_numpy(rng.standard_normal(C).astype(np.float16)).cuda()
-    gamma = rng.standard_normal(C).astype(np.float16); beta = rng.standard_normal(C).astype(np.float16)
-    y = torch.full_like(x, float("nan")); out = torch.full_like(x, float("nan"))
-    stats = torch.zeros(2 * G, device="cuda", dtype=torch.float64)
-    assert K.osb_channel_add_stats(x.data_ptr(), t.data_ptr(), y.data_ptr(), F16, C, HW, G, stats.data_ptr(), _stream()) == 0
+    rng = np.random.default_rng(seed)
+    gamma = rng.standard_normal(C).astype(NP[dtype]); beta = rng.standard_normal(C).astype(NP[dtype])
     tg, tb = torch.from_numpy(gamma).cuda(), torch.from_numpy(beta).cuda()
-    assert K.osb_group_norm_apply(y.data_ptr(), out.data_ptr(), F16, C, HW, G, tg.data_ptr(), tb.data_ptr(), 1e-5, 1, stats.data_ptr(), None, _stream()) == 0
+    out = torch.full_like(y, float("nan"))
+    clear = torch.ones(2 * G, device="cuda", dtype=torch.float64)
+    assert K.osb_group_norm_apply(y.data_ptr(), out.data_ptr(), dtype, C, HW, G, tg.data_ptr(), tb.data_ptr(), 1e-5, 1, stats.data_ptr(), clear.data_ptr(), _stream()) == 0
     torch.cuda.synchronize()
-    assert torch.equal(y, (x.float() + t.float()).half())
     ref, mean, rg = _gn_ref(y.double().cpu().numpy().reshape(-1), 1, C, HW, G, gamma.astype(np.float64), beta.astype(np.float64), 1)
-    _assert_within(out.cpu().numpy().reshape(-1), ref, _gn_tol(ref, mean, rg, F16), "channel_add_stats + apply, m = 1024")
+    _assert_within(out.cpu().numpy().reshape(-1), ref, _gn_tol(ref, mean, rg, dtype), what)
+    assert float(clear.abs().max()) == 0.0, f"{what}: the other slot was not cleared"
 
 
-@pytest.mark.xfail(reason="the conv epilogue gathers GroupNorm statistics as fp32 per-tile sums of y and y^2, which cancel in "
-                          "E[y^2] - mean^2 when the output mean is large against its spread", strict=False)
-def test_conv_epilogue_gn_stats_offset_mean(K):
-    """osb_conv2d_ex statistics + osb_group_norm_apply when the conv output sits at 1024 + O(1) (a large per-channel bias): GroupNorm of
-    the stored output against fp64.  Bar: _gn_tol (fp16)."""
+# HW, C, G: cpg 10, 4 (G = 64), 8 (G = 64) and 40; HW ragged against the CTA pixel strips
+CHANNEL_ADD_SHAPES = [(4096, 320, 32), (1000, 256, 64), (999, 512, 64), (333, 960, 24)]
+
+
+@pytest.mark.parametrize("m", STATS_M)
+@pytest.mark.parametrize("addv", [True, False], ids=["add", "stats-only"])
+@pytest.mark.parametrize("dtype", [F16, F32])
+@pytest.mark.parametrize("HW,C,G", CHANNEL_ADD_SHAPES)
+def test_channel_add_stats_offset_mean(K, HW, C, G, dtype, addv, m):
+    """osb_channel_add_stats (gn_stats_nhwc_vec_kernel): with addv, y = x + t[c] is written and its statistics gathered (a resnet's
+    time-embedding Add feeding a GroupNorm); without, the statistics of x (a GroupNorm whose producer gathered none).  x = m + 0.5 N(0,1)
+    per channel + N(0,1): the group mean is large against the spread at m >= 64.  The slot: _check_gn_slot; GroupNorm(+SiLU) of the
+    stored y from it: _gn_tol."""
     import torch
-    H = W = 32; Cin = Cout = 320; G = 32
-    g = torch.Generator(device="cuda").manual_seed(11)
+    rng = np.random.default_rng(HW + C + int(m) + 7 * dtype + int(addv))
+    xs = (m + 0.5 * rng.standard_normal((1, C)) + rng.standard_normal((HW, C))).astype(NP[dtype])
+    x = torch.from_numpy(xs).cuda()
+    stats = torch.zeros(2 * G, device="cuda", dtype=torch.float64)
+    if addv:
+        t = torch.from_numpy(rng.standard_normal(C).astype(NP[dtype])).cuda()
+        y = torch.full_like(x, float("nan"))
+        assert K.osb_channel_add_stats(x.data_ptr(), t.data_ptr(), y.data_ptr(), dtype, C, HW, G, stats.data_ptr(), _stream()) == 0
+        torch.cuda.synchronize()
+        assert torch.equal(y, (x.float() + t.float()).to(x.dtype))
+    else:
+        y = x
+        assert K.osb_channel_add_stats(x.data_ptr(), None, None, dtype, C, HW, G, stats.data_ptr(), _stream()) == 0
+        torch.cuda.synchronize()
+    what = f"channel_add_stats {'add' if addv else 'stats-only'} {'f16' if dtype == F16 else 'f32'} HW {HW} C {C} G {G} m {m}"
+    _check_gn_slot(stats, y.double().cpu().numpy(), HW, C, G, what)
+    _check_gn_apply_from_slot(K, y, stats, dtype, HW, C, G, HW + C, what)
+
+
+# route, forced (bm, bn, split) or None, CTA-pair mode, Cout, G: every EXTRAS tile, the CTA pairs and the split-K reduce, with cpg
+# 10, 4, 8 and 40 spread over them
+CONV_STATS_ROUTES = [
+    ("tile-128x128", (128, 128, 1), 1, 320, 32),
+    ("tile-128x64", (128, 64, 1), 1, 256, 64),
+    ("tile-128x80", (128, 80, 1), 1, 320, 8),
+    ("tile-128x160", (128, 160, 1), 1, 320, 32),
+    ("tile-64x64", (64, 64, 1), 1, 136, 17),
+    ("tile-64x128", (64, 128, 1), 1, 256, 64),
+    ("tile-64x160", (64, 160, 1), 1, 320, 8),
+    ("cta-pair", None, 2, 320, 32),
+    ("split-k", (128, 128, 3), 1, 320, 8),
+    ("split-k", (64, 128, 2), 1, 256, 64),
+]
+
+
+@pytest.mark.parametrize("m", STATS_M)
+@pytest.mark.parametrize("route,force,pair,Cout,G", CONV_STATS_ROUTES, ids=[f"{r[0]}-cpg{r[3] // r[4]}" for r in CONV_STATS_ROUTES])
+def test_conv_epilogue_gn_stats_offset_mean(K, route, force, pair, Cout, G, m):
+    """osb_conv2d_ex with statistics: the tile epilogue (gn_stats_pair) at every EXTRAS tile, forced with osb_tc_set_tile and pinned by
+    the launch profile, through CTA pairs, and the split-K reduce kernel -- the conv output sits at m + O(1) through a large bias (and a
+    residual: half of m each in the split-K cases, so the reduce kernel adds both).  On a 25 x 19 image every tile is ragged and some
+    warps hold no valid row.  The slot: _check_gn_slot; GroupNorm(+SiLU) of the stored output from it: _gn_tol (fp16)."""
+    import torch
+    from test_tc_tiles_gpu import _profile
+    ci = ctypes.c_int
+    K.osb_tc_set_tile.argtypes = [ci] * 3
+    K.osb_tc_set_pair_mode.argtypes = [ci]
+    H, W, Cin = 25, 19, 64
+    g = torch.Generator(device="cuda").manual_seed(Cout * 7 + G + int(m))
     x = torch.randn(H, W, Cin, device="cuda", generator=g).half()
     w = (torch.randn(Cout, 3, 3, Cin, device="cuda", generator=g) / (9 * Cin) ** 0.5).half()
-    bias = (1024.0 + torch.randn(Cout, device="cuda", generator=g)).half()
+    split = force is not None and force[2] > 1
+    bias = ((m / 2 if split else m) + 0.5 * torch.randn(Cout, device="cuda", generator=g)).half()
+    bias2 = torch.randn(Cout, device="cuda", generator=g).half()
+    res = (m / 2 + torch.randn(H, W, Cout, device="cuda", generator=g)).half() if split else None
     y = torch.full((H, W, Cout), float("nan"), device="cuda", dtype=torch.half)
     stats = torch.zeros(2 * G, device="cuda", dtype=torch.float64)
-    done = ctypes.c_int(0)
-    assert K.osb_conv2d_ex(x.data_ptr(), w.data_ptr(), bias.data_ptr(), None, None, y.data_ptr(), H, W, Cin, Cout, 3, 3, 1, 1, 1, H, W, F16, 0,
-                           _stream(), stats.data_ptr(), G, ctypes.byref(done)) == 0
+    done = ci(0)
+    if force:
+        K.osb_tc_set_tile(*force)
+    K.osb_tc_set_pair_mode(pair)
+    try:
+        prof = _profile(K, lambda: K.osb_conv2d_ex(x.data_ptr(), w.data_ptr(), bias.data_ptr(), bias2.data_ptr(), res.data_ptr() if split else None,
+                                                   y.data_ptr(), H, W, Cin, Cout, 3, 3, 1, 1, 1, H, W, F16, 2 if force else 0, _stream(),
+                                                   stats.data_ptr(), G, ctypes.byref(done)))
+    finally:
+        K.osb_tc_set_tile(0, 0, 0)
+        K.osb_tc_set_pair_mode(1)
     torch.cuda.synchronize()
-    assert done.value == 1
-    gamma = torch.randn(Cout, device="cuda", generator=g).half(); beta = torch.randn(Cout, device="cuda", generator=g).half()
-    out = torch.full_like(y, float("nan"))
-    assert K.osb_group_norm_apply(y.data_ptr(), out.data_ptr(), F16, Cout, H * W, G, gamma.data_ptr(), beta.data_ptr(), 1e-5, 1, stats.data_ptr(), None, _stream()) == 0
-    torch.cuda.synchronize()
-    ref, mean, rg = _gn_ref(y.double().cpu().numpy().reshape(-1), 1, Cout, H * W, G, gamma.double().cpu().numpy(), beta.double().cpu().numpy(), 1)
-    _assert_within(out.cpu().numpy().reshape(-1), ref, _gn_tol(ref, mean, rg, F16), "conv epilogue statistics, m = 1024")
+    assert len(prof) == 1, prof
+    if force:
+        assert (prof[0]["bm"], prof[0]["bn"], prof[0]["split"]) == force, prof
+    else:
+        assert (prof[0]["bm"], prof[0]["bn"], prof[0]["split"]) == (128, 128, 1), prof
+    assert done.value == 1, "the kernel did not report the statistics"
+    what = f"conv epilogue {route} Cout {Cout} G {G} m {m}"
+    _check_gn_slot(stats, y.double().cpu().numpy(), H * W, Cout, G, what)
+    _check_gn_apply_from_slot(K, y, stats, F16, H * W, Cout, G, Cout + G, what)
 
 
 @pytest.mark.parametrize("dtype", [F16, F32])
