@@ -237,6 +237,18 @@ int osb_sdpa_flash_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d
 int osb_sdpa_flash(const void* q, const void* k, const void* v, const void* mask, void* out,
                    int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, float scale, void* stream);
 
+/* osb_sdpa_flash for fp32 (d % 8 == 0, 8 <= d <= 128, dv == d) on the bf16 tensor cores at fp32 accuracy, with the numerics of
+ * osb_flash_attention_f32x: q, k and v are split into three bf16 planes each, Q K^T and P V sum the six significant cross products in
+ * fp32, the softmax is fp32 with an exact running maximum over the logits s * scale + mask (natural units: a mask of -3.4028235e38 is
+ * kept finite).  Same layouts as osb_sdpa_flash with fp32 elements and an fp32 mask; any finite scale.  A row whose keys are all -inf
+ * up to some key tile ignores those tiles.  `planes`: device scratch of 6 * (Hq * Tq + 2 * Hkv * Tk) * d bytes (16-byte aligned) for the
+ * bf16 planes, written by the launch.  The launch returns cudaErrorInvalidValue and enqueues nothing for anything *_ok refuses, for q,
+ * k, v, out or planes not 16-byte aligned, a mask not 4-byte aligned and a scale that is not finite. */
+int osb_sdpa_flash_f32x_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, int dtype);
+int osb_sdpa_flash_f32x(const void* q, const void* k, const void* v, const void* mask, void* out,
+                        int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, float scale,
+                        void* planes, void* stream);
+
 /* qu8 GEMM / conv with XNNPACK's requantisation (bit-exact target; SURVEY section 8c):
  * acc = sum (x - zx)(w - zw) + bias_i32; y = clamp(lrintf(acc * (sx*sw/sy)) + zy, 0, 255). */
 int osb_gemm_qu8(const uint8_t* A, const uint8_t* B, uint8_t* C, const int32_t* bias, int64_t M, int64_t N, int64_t K,

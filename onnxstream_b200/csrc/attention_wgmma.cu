@@ -19,6 +19,7 @@
 // flash_attention_wide_kernel (below): 160 < d <= 512 -- the VAE decoder's single-head d = 512 attention -- with O split over its columns.
 // flash_attention_f32x_kernel (below): fp32 q / k / v / out on bf16 wgmma through the triple split, d <= 160.
 // flash_attention_wide_f32x_kernel (below): the wide kernel's slices with the f32x kernel's numerics, fp32 and 160 < d <= 512.
+// sdpa_flash_f32x_kernel (below): sdpa_flash_kernel's grouped-KV masked attention with the f32x kernel's numerics, fp32 and d <= 128.
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -804,19 +805,28 @@ __global__ void f32x_split_kernel(const float* __restrict__ q, int64_t ldq, cons
     }
 }
 
-// Online softmax of one score tile for the fp32 kernel: fa_softmax with fp32 arithmetic -- the logit s * scale rounded once, as fp32
+// Online softmax of one score tile for the fp32 kernels: fa_softmax with fp32 arithmetic -- the logit s * scale rounded once, as fp32
 // attention rounds it, and expf instead of the one-MUFU ex2 (whose ~2^-22 relative error and the rounding of scale * log2e show at fp32
 // accuracy); the exact running maximum.  Padding keys (last tile only) get -inf.
-template <int BK>
-__device__ __forceinline__ void f32x_softmax(float (&s)[BK / 2], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2], int key0, int cq, int Tk, float scale)
+// MASK: the logit is s * scale + mask in natural units, rounded as fp32 attention rounds the two steps; mk[h][c] holds the mask of this
+// thread's row r + 8h at the columns 8c + cq, + 1.  The running maximum is then taken over the masked, scaled logits (any finite scale),
+// and a tile whose logits so far are all -inf (a -inf mask over a row's first keys) leaves m_run, l_run and O as they are.
+template <int BK, bool MASK = false>
+__device__ __forceinline__ void f32x_softmax(float (&s)[BK / 2], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2], int key0, int cq, int Tk, float scale,
+                                             const float2 (*mk)[BK / 8] = nullptr)
 {
 #pragma unroll
     for (int c = 0; c < BK / 8; c++)
 #pragma unroll
         for (int e = 0; e < 2; e++) {
             const bool pad = key0 + 8 * c + cq + e >= Tk;
-            s[4 * c + e] = pad ? -INFINITY : s[4 * c + e] * scale;
-            s[4 * c + 2 + e] = pad ? -INFINITY : s[4 * c + 2 + e] * scale;
+            if constexpr (MASK) {
+                s[4 * c + e] = pad ? -INFINITY : __fmul_rn(s[4 * c + e], scale) + (e ? mk[0][c].y : mk[0][c].x);
+                s[4 * c + 2 + e] = pad ? -INFINITY : __fmul_rn(s[4 * c + 2 + e], scale) + (e ? mk[1][c].y : mk[1][c].x);
+            } else {
+                s[4 * c + e] = pad ? -INFINITY : s[4 * c + e] * scale;
+                s[4 * c + 2 + e] = pad ? -INFINITY : s[4 * c + 2 + e] * scale;
+            }
         }
     float m_new[2];
 #pragma unroll
@@ -824,6 +834,10 @@ __device__ __forceinline__ void f32x_softmax(float (&s)[BK / 2], float (&m_run)[
         m_new[h] = fmaxf(m_run[h], fa_row_max<BK>(s, h));
         alpha[h] = expf(m_run[h] - m_new[h]);                        // 0 on the first tile (m_run = -inf)
         m_run[h] = m_new[h];
+        if constexpr (MASK) {
+            // every logit so far -inf: p = expf(-inf - 0) = 0 and alpha = 1 instead of the NaN of -inf - -inf
+            if (m_new[h] == -INFINITY) { alpha[h] = 1.f; m_new[h] = 0.f; }
+        }
     }
     float lsum[2] = { 0.f, 0.f };
 #pragma unroll
@@ -1268,6 +1282,211 @@ int wx_launch(const float* q, const float* k, const float* v, float* out, FaPara
     return fa_launch_kernel<flash_attention_wide_f32x_kernel>(grid, WD_THREADS, WX_SMEM, st, mq, mk, mv, p, scale, out);
 }
 
+// ---- fp32 grouped-KV masked attention on the tensor cores (ScaledDotProductAttention in fp32 arithmetic: prompt prefill) -------------
+// softmax(Q K^T * scale + mask) V of sdpa_flash_kernel for fp32 q [Hq, Tq, d], k / v [Hkv, Tk, d], mask [Tq, Tk], out [Hq, Tq, d], with
+// the numerics of flash_attention_f32x_kernel: bf16 planes x = h + m + l, six cross products, small ones first, the fp32
+// softmax with the mask added in natural units (f32x_softmax<BK, true>).  Roles and packing are sdpa_flash_kernel's: one CTA per 128
+// packed rows [G*Tq, d] of one KV head (grid.y), packed row R is query R % Tq of head hk*G + R / Tq and reads mask row R % Tq; a TMA
+// producer warp and two consumer warpgroups at 232 registers, unpipelined.  Tiles as the f32x kernel's (FaCfg<NCH, BK, QKS, KS, 3>):
+// d <= 64: 64-key tiles, 2 stages; d <= 128: 32-key tiles, 2 stages.
+// Planes as the wide fp32 kernel lays them out: q and v [rows][3][d] read through (3 d, rows, Hkv) maps, K [Hkv][3][Tk][d] through a
+// (d, Tk, 3 Hkv) map.  Rows past G*Tq and keys past Tk are zero-filled by TMA; a Q chunk that ends past d reads the next plane's first
+// columns, which meet K's zero-filled columns, and a V chunk's columns past d feed output columns that are never stored.
+// The mask is not folded into log2 units: llm.cpp's fp32 masks hold -3.4028235e38, which times log2e overflows to -inf.
+struct SdpaF32xParams {
+    int rows;                // G * Tq: packed query rows per KV head
+    int Tq, Tk, d;
+    int kv_tiles;
+    float scale;
+    const float* mask;       // [Tq, Tk] additive, or nullptr
+    int mask_vec;            // 8-byte mask loads: Tk even and the mask 8-byte aligned
+    float* out;              // [Hkv][G*Tq][d] (= [Hq, Tq, d])
+};
+
+// mask[row][col], mask[row][col + 1]; keys past Tk read as 0 (they get -inf afterwards).  vec: the pair is 8-byte aligned.
+__device__ __forceinline__ float2 ld_mask_pair_f32(const float* row, int col, int Tk, bool vec)
+{
+    if (col + 1 < Tk) {
+        if (vec) return __ldg(reinterpret_cast<const float2*>(row + col));
+        return make_float2(__ldg(row + col), __ldg(row + col + 1));
+    }
+    return make_float2(col < Tk ? __ldg(row + col) : 0.f, 0.f);
+}
+
+template <int NCH, int BK, int QKS, int KS>
+__global__ void __launch_bounds__(FA_THREADS, 1)
+sdpa_flash_f32x_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+                       const SdpaF32xParams p)
+{
+    using C = FaCfg<NCH, BK, QKS, KS, 3>;
+    osb_pdl_trigger_entry();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int r0 = blockIdx.x * BQ, hk = blockIdx.y;
+    const int n_kv = p.kv_tiles;
+    uint8_t* smem = fa_prologue(&map_q, &map_k, &map_v, C::BARS, FA_CONSUMERS / 32, KS);   // kv_empty: one arrival per consumer warp
+    uint8_t* sQ = smem;
+    uint8_t* sK = sQ + C::Q_BYTES;
+    uint8_t* sV = sK + KS * C::KV_BYTES;
+    uint64_t* q_full = (uint64_t*)(smem + C::BARS);   // [1]
+    uint64_t* kv_full = q_full + 1;                    // [KS]
+    uint64_t* kv_empty = kv_full + KS;                 // [KS]
+
+    if (warp < 4) {
+        setmaxnreg_dec<FA_PRODUCER_REGS>();
+        if (warp == 0) {
+            if (elect_one()) {
+                mbar_expect_tx(q_full, C::Q_BYTES);
+#pragma unroll
+                for (int pl = 0; pl < 3; pl++)
+#pragma unroll
+                    for (int c = 0; c < NCH; c++) tma_load_3d(sQ + pl * C::Q_PLANE + c * C::Q_CHUNK, &map_q, q_full, pl * p.d + 64 * c, r0, hk);
+            }
+            __syncwarp();
+            fa_produce_kv<KS>(kv_full, kv_empty, n_kv, 2 * C::KV_BYTES, [&](int st, int j, uint64_t* bar) {
+#pragma unroll
+                for (int pl = 0; pl < 3; pl++)
+#pragma unroll
+                    for (int c = 0; c < NCH; c++) {
+                        const int off = st * C::KV_BYTES + pl * C::KV_PLANE + c * C::KV_CHUNK;
+                        tma_load_3d(sK + off, &map_k, bar, 64 * c, j * BK, 3 * hk + pl);
+                        tma_load_3d(sV + off, &map_v, bar, pl * p.d + 64 * c, j * BK, hk);
+                    }
+            });
+        }
+    } else {
+        // ===================== warpgroups 1, 2: 64 packed rows each =====================
+        setmaxnreg_inc<FA_CONSUMER_REGS>();
+        const int wg = (warp >> 2) - 1;
+        const int r = (warp & 3) * 16 + (lane >> 2);
+        const int cq = 2 * (lane & 3);
+        const uint64_t qdesc = make_smem_desc(smem_u32(sQ) + wg * (BQ / 2) * 128, 16, 1024);
+        const uint64_t kdesc0 = make_smem_desc(smem_u32(sK), 16, 1024);
+        const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), C::KV_CHUNK, 1024);
+        const bool has_mask = p.mask != nullptr, vec = p.mask_vec != 0;
+        const float* mrow[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int R = r0 + wg * (BQ / 2) + r + 8 * h;                     // rows past G*Tq (zero-filled by TMA) are never stored
+            mrow[h] = has_mask ? p.mask + (long long)(R % p.Tq) * p.Tk : nullptr;
+        }
+        float o[NCH][32];
+#pragma unroll
+        for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+            for (int i = 0; i < 32; i++) o[ch][i] = 0.f;
+        float m_run[2] = { -INFINITY, -INFINITY }, l_run[2] = { 0.f, 0.f }, alpha[2];
+        mbar_wait(q_full, 0);
+        for (int j = 0; j < n_kv; j++) {
+            const int st = j % KS;
+            const int key0 = j * BK;
+            mbar_wait(&kv_full[st], (j / KS) & 1);
+            // S = the six cross products, small ones first, as in flash_attention_f32x_kernel
+            const uint64_t kdesc = kdesc0 + (uint64_t)(st * C::KV_BYTES >> 4), vdesc = vdesc0 + (uint64_t)(st * C::KV_BYTES >> 4);
+            float s[BK / 2];
+            fence_regs(s);
+            wgmma_fence();
+#pragma unroll
+            for (int xx = 0; xx < 6; xx++)
+#pragma unroll
+                for (int k = 0; k < QKS; k++) {
+                    const int x = 5 - xx;
+                    qk_mma_bf16<BK>(s, qdesc + (uint64_t)(((x3a(x) * C::Q_PLANE + (k >> 2) * C::Q_CHUNK) >> 4) + (k & 3) * 2),
+                                    kdesc + (uint64_t)(((x3b(x) * C::KV_PLANE + (k >> 2) * C::KV_CHUNK) >> 4) + (k & 3) * 2), (k | xx) != 0);
+                }
+            wgmma_commit();
+            // the mask loads (L2-resident: every head reads the same [Tq, Tk] block) are in flight while the MMAs run
+            float2 mk[2][BK / 8];
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int c = 0; c < BK / 8; c++) mk[h][c] = has_mask ? ld_mask_pair_f32(mrow[h], key0 + 8 * c + cq, p.Tk, vec) : make_float2(0.f, 0.f);
+            wgmma_wait<0>();
+            fence_regs(s);
+            f32x_softmax<BK, true>(s, m_run, l_run, alpha, key0, cq, p.Tk, p.scale, mk);
+            // O *= alpha; P -> three bf16 planes; O += P V one 64-column chunk at a time through a fresh register tile added in fp32
+#pragma unroll
+            for (int ch = 0; ch < NCH; ch++)
+#pragma unroll
+                for (int c = 0; c < 8; c++)
+#pragma unroll
+                    for (int h = 0; h < 2; h++) { o[ch][4 * c + 2 * h] *= alpha[h]; o[ch][4 * c + 2 * h + 1] *= alpha[h]; }
+            uint32_t a[3][BK / 16][4];
+#pragma unroll
+            for (int c = 0; c < BK / 8; c++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    __nv_bfloat16 p0[3], p1[3];
+                    bf16x3_split(s[4 * c + 2 * h], p0[0], p0[1], p0[2]);
+                    bf16x3_split(s[4 * c + 2 * h + 1], p1[0], p1[1], p1[2]);
+#pragma unroll
+                    for (int pl = 0; pl < 3; pl++) a[pl][c >> 1][(c & 1) * 2 + h] = pack_bf162(p0[pl], p1[pl]);
+                }
+#pragma unroll
+            for (int pl = 0; pl < 3; pl++) fence_regs(a[pl]);
+#pragma unroll
+            for (int ch = 0; ch < NCH; ch++) {
+                float t[32];
+                fence_regs(t);
+                wgmma_fence();
+#pragma unroll
+                for (int xx = 0; xx < 6; xx++)
+#pragma unroll
+                    for (int kk = 0; kk < BK / 16; kk++) {
+                        const int x = 5 - xx;
+                        wgmma_m64n64k16_bf16_rs(t, a[x3a(x)][kk], vdesc + (uint64_t)((x3b(x) * C::KV_PLANE + ch * C::KV_CHUNK + kk * 2048) >> 4), (kk | xx) != 0);
+                    }
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(t);
+#pragma unroll
+                for (int i = 0; i < 32; i++) o[ch][i] += t[i];
+            }
+#pragma unroll
+            for (int pl = 0; pl < 3; pl++) fence_regs(a[pl]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&kv_empty[st]);
+        }
+        // out[hk][R][col]
+        float* rows[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int R = r0 + wg * (BQ / 2) + r + 8 * h;
+            rows[h] = R < p.rows ? p.out + ((long long)hk * p.rows + R) * p.d : nullptr;
+        }
+        fa_store(o, l_run, rows, p.d, cq);
+    }
+}
+
+// Every tensor map is made before the splits are enqueued.  planes: pq [Hq * Tq][3][d], pk [Hkv][3][Tk][d], pv [Hkv * Tk][3][d].
+template <int NCH, int BK, int QKS, int KS>
+int sdpa_f32x_launch(const float* q, const float* k, const float* v, SdpaF32xParams p, int64_t Hkv, __nv_bfloat16* planes, cudaStream_t st)
+{
+    using Cf = FaCfg<NCH, BK, QKS, KS, 3>;
+    const int64_t rows = p.rows, Tk = p.Tk, d = p.d;
+    __nv_bfloat16* pq = planes;
+    __nv_bfloat16* pk = pq + 3 * Hkv * rows * d;
+    __nv_bfloat16* pv = pk + 3 * Hkv * Tk * d;
+    CUtensorMap mq, mk, mv;
+    if (!make_map(&mq, pq, 3 * d, rows, Hkv, 3 * d * 2, rows * 3 * d * 2, 64, BQ, 1) ||
+        !make_map(&mk, pk, d, Tk, 3 * Hkv, d * 2, Tk * d * 2, 64, BK, 1) ||
+        !make_map(&mv, pv, 3 * d, Tk, Hkv, 3 * d * 2, Tk * 3 * d * 2, 64, BK, 1))
+        return (int)cudaErrorInvalidValue;
+    // q and v as [rows, d] with no K part, then K
+    osb_launch((f32x_split_kernel), grid_for((size_t)(Hkv * rows * d / 4), 256), 256, 0, st, q, d, q, d, q, d, pq, pq, pq, Hkv * rows,
+               (int64_t)0, (int)d);
+    int e = launched();
+    if (e) return e;
+    osb_launch((f32x_split_kernel), grid_for((size_t)(Hkv * Tk * d / 4), 256), 256, 0, st, v, d, v, d, v, d, pv, pv, pv, Hkv * Tk,
+               (int64_t)0, (int)d);
+    if ((e = launched())) return e;
+    const dim3 kgrid((unsigned)((Tk + 31) / 32), (unsigned)((d + 31) / 32), (unsigned)Hkv), kblock(32, 8);
+    osb_launch((f32x_split_k_kernel<false>), kgrid, kblock, 0, st, k, pk, (int)Tk, (int)d);
+    if ((e = launched())) return e;
+    p.kv_tiles = (int)((Tk + BK - 1) / BK);
+    dim3 grid((unsigned)((rows + BQ - 1) / BQ), (unsigned)Hkv);
+    return fa_launch_kernel<sdpa_flash_f32x_kernel<NCH, BK, QKS, KS>>(grid, FA_THREADS, Cf::SMEM, st, mq, mk, mv, p);
+}
+
 }  // namespace
 
 extern "C" int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
@@ -1386,4 +1605,33 @@ extern "C" int osb_sdpa_flash(const void* q, const void* k, const void* v, const
     p.mask = (const __half*)mask; p.out = (__half*)out;
     cudaStream_t st = (cudaStream_t)stream;
     return d <= 64 ? sdpa_launch<1, 128>(q, k, v, p, Hkv, st) : sdpa_launch<2, 64>(q, k, v, p, Hkv, st);
+}
+
+extern "C" int osb_sdpa_flash_f32x_ok(int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, int64_t dv, int dtype)
+{
+    return dtype == OSB_F32 && d == dv && d >= 8 && d <= 128 && d % 8 == 0 && Hkv >= 1 && Hkv <= 65535 && Hq >= Hkv && Hq % Hkv == 0 &&
+           Tq >= 1 && Tk >= 1 && (Hq / Hkv) * Tq <= (int64_t)INT32_MAX - BQ && Tk <= (int64_t)INT32_MAX - BKV && get_encode() != nullptr;
+}
+
+// osb_sdpa_flash for fp32 q / k / v / mask / out (contiguous; q, k, v, out and planes 16-byte aligned, the mask 4-byte aligned) on the
+// bf16 tensor cores at fp32 accuracy.  Any finite scale.  planes: scratch of 6 (Hq Tq + 2 Hkv Tk) d bytes.  Four launches: the splits of
+// q, v and k, then the attention.
+extern "C" int osb_sdpa_flash_f32x(const void* q, const void* k, const void* v, const void* mask, void* out,
+                                   int64_t Hq, int64_t Hkv, int64_t Tq, int64_t Tk, int64_t d, float scale, void* planes, void* stream)
+{
+    if (!osb_sdpa_flash_f32x_ok(Hq, Hkv, Tq, Tk, d, d, OSB_F32) || !(fabsf(scale) < INFINITY)) return (int)cudaErrorInvalidValue;
+    if (!aligned16(q, k, v, out, planes) || ((uintptr_t)mask & 3) != 0) return (int)cudaErrorInvalidValue;
+    SdpaF32xParams p{};
+    p.rows = (int)((Hq / Hkv) * Tq); p.Tq = (int)Tq; p.Tk = (int)Tk; p.d = (int)d;
+    p.scale = scale;
+    p.mask = (const float*)mask;
+    p.mask_vec = (Tk % 2 == 0) && ((uintptr_t)mask & 7) == 0;
+    p.out = (float*)out;
+    const float* fq = (const float*)q; const float* fk = (const float*)k; const float* fv = (const float*)v;
+    __nv_bfloat16* pl = (__nv_bfloat16*)planes;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (d <= 48) return sdpa_f32x_launch<1, 64, 3, 2>(fq, fk, fv, p, Hkv, pl, st);
+    if (d <= 64) return sdpa_f32x_launch<1, 64, 4, 2>(fq, fk, fv, p, Hkv, pl, st);
+    if (d <= 80) return sdpa_f32x_launch<2, 32, 5, 2>(fq, fk, fv, p, Hkv, pl, st);
+    return sdpa_f32x_launch<2, 32, 8, 2>(fq, fk, fv, p, Hkv, pl, st);
 }

@@ -1985,6 +1985,15 @@ void Engine::Impl::fused_sdpa(const Step& s)
         push(i + 5, 0, out);
         return;
     }
+    // fp32 arithmetic: the same grouped-KV flash attention on the bf16 tensor cores at fp32 accuracy, for grouped and equal head counts
+    // alike (instead of the per-row kernel, or the GEMM -> softmax -> GEMM chain and its fp32 [Hq, Tq, Tk] score buffer)
+    if (q.type == DType::f32 && Tq > 16 && D == Dv && flash_on() && aligned && osb_sdpa_flash_f32x_ok(Hq, Hkv, Tq, Tk, D, Dv, K(q.type))) {
+        // the launch splits q, k, v into bf16 planes (6 bytes per element) in this scratch
+        Tensor planes = make(DType::f16, { 3 * (Hq * Tq + 2 * Hkv * Tk) * D });
+        ck(osb_sdpa_flash_f32x(q.data(), k.data(), v.data(), m.data(), out.mdata(), Hq, Hkv, Tq, Tk, D, scale, planes.mdata(), st), "osb_sdpa_flash_f32x");
+        push(i + 5, 0, out);
+        return;
+    }
     attention_core(q3, k3, v3, scale, false, &m, Hq / Hkv, o3);
     push(i + 5, 0, out);
 }

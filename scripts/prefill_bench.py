@@ -1,6 +1,9 @@
 #!/usr/bin/env python
 """scripts/prefill_bench.py -- prompt prefill on the GPU: the grouped-KV masked flash attention kernel (osb_sdpa_flash) against the
 per-row kernel it replaces (osb_attention), and the TinyLlama-1.1B-shaped prefill step end to end with b200_flash_attention on and off.
+--f32: the same for fp32 arithmetic -- osb_sdpa_flash_f32x (its three plane splits included) against osb_attention in fp32 (at Tq <= 128
+with Tk >= 256 that is the split-KV decode kernel), with short chat turns (Tq 17..128 over Tk 2048) added, and the model step without
+use_fp16_arithmetic.
 
 Prints ONE JSON line: the card (name, power limit, max SM clock, read with an nvidia-smi query), then
   kernel: per shape, ms per launch (CUDA events over --iters launches after warm-up) for both kernels, TFLOP/s as 4*Hq*Tq*Tk*d / t
@@ -28,7 +31,7 @@ sys.path.insert(0, ROOT)
 from onnxstream_b200 import emit  # noqa: E402
 from onnxstream_b200.model import ENGINE_LIB, Model  # noqa: E402
 
-F16 = 2
+F16, F32 = 2, 3
 KERNEL_SHAPES = [
     # name, Hq, Hkv, Tq, Tk, d
     ("tinyllama_512", 32, 4, 512, 512, 64),
@@ -37,6 +40,14 @@ KERNEL_SHAPES = [
     ("mistral_512", 32, 8, 512, 512, 128),
     ("mistral_2048", 32, 8, 2048, 2048, 128),
     ("mistral_turn_128x2048", 32, 8, 128, 2048, 128),
+]
+# fp32 only: short turns, where osb_attention takes its split-KV decode kernel
+F32_TURN_SHAPES = [
+    ("tinyllama_turn_17x2048", 32, 4, 17, 2048, 64),
+    ("tinyllama_turn_32x2048", 32, 4, 32, 2048, 64),
+    ("tinyllama_turn_64x2048", 32, 4, 64, 2048, 64),
+    ("mistral_turn_17x2048", 32, 8, 17, 2048, 128),
+    ("mistral_turn_64x2048", 32, 8, 64, 2048, 128),
 ]
 MODEL_CASES = [(512, 0), (2048, 0), (128, 1920)]     # (new tokens, cached positions)
 UPCAST = ("layernorm", "/norm/")
@@ -48,31 +59,39 @@ def card():
     return {"name": name, "power_limit": power, "max_sm_clock": clock}
 
 
-def kernel_level(iters, warmup):
+def kernel_level(iters, warmup, f32=False):
     import torch
     lib = ctypes.CDLL(ENGINE_LIB)
     vp, i64, cf, ci = ctypes.c_void_p, ctypes.c_int64, ctypes.c_float, ctypes.c_int
     lib.osb_sdpa_flash.argtypes = [vp] * 5 + [i64] * 5 + [cf, vp]
+    lib.osb_sdpa_flash_f32x.argtypes = [vp] * 5 + [i64] * 5 + [cf, vp, vp]
     lib.osb_attention.argtypes = [vp] * 5 + [i64] * 5 + [cf, ci, i64, ci, vp]
     stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    dt = torch.float32 if f32 else torch.half
     out = []
-    for name, Hq, Hkv, Tq, Tk, d in KERNEL_SHAPES:
+    for name, Hq, Hkv, Tq, Tk, d in KERNEL_SHAPES + (F32_TURN_SHAPES if f32 else []):
         g = torch.Generator(device="cuda").manual_seed(Hq * Tq + Tk + d)
-        q = torch.randn(Hq, Tq, d, device="cuda", generator=g).half()
-        k = torch.randn(Hkv, Tk, d, device="cuda", generator=g).half()
-        v = torch.randn(Hkv, Tk, d, device="cuda", generator=g).half()
+        q = torch.randn(Hq, Tq, d, device="cuda", generator=g).to(dt)
+        k = torch.randn(Hkv, Tk, d, device="cuda", generator=g).to(dt)
+        v = torch.randn(Hkv, Tk, d, device="cuda", generator=g).to(dt)
         past = Tk - Tq
         keep = torch.arange(Tk, device="cuda")[None, :] <= past + torch.arange(Tq, device="cuda")[:, None]
-        mask = torch.where(keep, 0.0, -65504.0).half()
+        mask = torch.where(keep, 0.0, -65504.0).to(dt)
         scale = 1.0 / d ** 0.5
-        o_new = torch.empty(Hq, Tq, d, device="cuda", dtype=torch.half)
+        o_new = torch.empty(Hq, Tq, d, device="cuda", dtype=dt)
         o_old = torch.empty_like(o_new)
+        planes = torch.empty(3 * (Hq * Tq + 2 * Hkv * Tk) * d, device="cuda", dtype=torch.bfloat16) if f32 else None
 
         def new():
-            assert lib.osb_sdpa_flash(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr(), o_new.data_ptr(), Hq, Hkv, Tq, Tk, d, scale, stream) == 0
+            if f32:
+                assert lib.osb_sdpa_flash_f32x(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr(), o_new.data_ptr(), Hq, Hkv, Tq, Tk, d, scale,
+                                               planes.data_ptr(), stream) == 0
+            else:
+                assert lib.osb_sdpa_flash(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr(), o_new.data_ptr(), Hq, Hkv, Tq, Tk, d, scale, stream) == 0
 
         def old():
-            assert lib.osb_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr(), o_old.data_ptr(), Hq, Tq, Tk, d, d, scale, 0, Hq // Hkv, F16, stream) == 0
+            assert lib.osb_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr(), o_old.data_ptr(), Hq, Tq, Tk, d, d, scale, 0, Hq // Hkv,
+                                     F32 if f32 else F16, stream) == 0
 
         def timed(fn):
             for _ in range(warmup):
@@ -91,12 +110,12 @@ def kernel_level(iters, warmup):
                     "flash_ms": round(t_new, 4), "rows_kernel_ms": round(t_old, 4),
                     "flash_tflops": round(flop / t_new / 1e9, 2), "rows_kernel_tflops": round(flop / t_old / 1e9, 3),
                     "speedup": round(t_old / t_new, 1), "max_abs_diff": float((o_new.float() - o_old.float()).abs().max())})
-        del q, k, v, mask, o_new, o_old
+        del q, k, v, mask, o_new, o_old, planes
         torch.cuda.empty_cache()
     return out
 
 
-def model_level(reps, warmup):
+def model_level(reps, warmup, f32=False):
     out = []
     for T, past in MODEL_CASES:
         cfg = emit.LlamaConfig(past=past)
@@ -107,7 +126,7 @@ def model_level(reps, warmup):
             models = {}
             for flash in (1, 0):
                 m = Model(ENGINE_LIB, 0, "ram+nocache")
-                for o in ("use_fp16_arithmetic", "use_scaled_dp_attn_op") + (("support_dynamic_shapes",) if past == 0 else ()):
+                for o in ("use_scaled_dp_attn_op",) + (() if f32 else ("use_fp16_arithmetic",)) + (("support_dynamic_shapes",) if past == 0 else ()):
                     m.set_option(o, True)
                 for p in UPCAST:
                     m.add_upcast_pattern(p)
@@ -154,13 +173,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--reps", type=int, default=5, help="timed model runs per setting (alternated)")
     ap.add_argument("--skip-model", action="store_true")
+    ap.add_argument("--f32", action="store_true", help="fp32 arithmetic: osb_sdpa_flash_f32x against osb_attention in fp32, short turns added")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         sys.exit("prefill_bench.py needs a CUDA device")
-    res = {"card": card(), "kernel": kernel_level(a.iters, a.warmup)}
+    res = {"card": card(), "dtype": "float32" if a.f32 else "float16", "kernel": kernel_level(a.iters, a.warmup, a.f32)}
     if not a.skip_model:
-        res["model"] = model_level(a.reps, 2)
+        res["model"] = model_level(a.reps, 2, a.f32)
     print(json.dumps(res))
 
 
