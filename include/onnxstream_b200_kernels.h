@@ -87,6 +87,10 @@ int osb_group_norm(const void* x, void* y, int dtype, int nhwc, int64_t C, int64
 /* GEGLU feed-forward gate: x [rows, 2*inner] -> y [rows, inner], y = x[:, :inner] * gelu_erf(x[:, inner:]).  One pass for the
  * Slice, Slice, Div, Erf, Add, Mul, Mul, Mul group (src/onnxstream.cpp Slice 6499-6652, Erf 1950-2100, binary ops 1666-1949). */
 int osb_geglu(const void* x, void* y, int dtype, int64_t rows, int64_t inner, void* stream);
+/* The feed-forward MatMul + bias and the GEGLU gate in one tensor-core launch (fp16): y [M, inner] = the osb_geglu of A [M, K] . B [K, 2 inner]
+ * + bias [2 inner] (bias may be NULL), bit-identical to the unsplit GEMM followed by osb_geglu.  cudaErrorNotSupported (801): inner % 64 != 0,
+ * or a shape / alignment outside the tensor-core path. */
+int osb_tc_gemm_geglu(const void* A, const void* B, void* y, const void* bias, int64_t M, int64_t inner, int64_t K, void* stream);
 
 /* Fused LayerNorm over the last axis (ReduceMean,Sub,Pow,ReduceMean,Add,Sqrt,Div,Mul,Add chain; src/onnxstream.cpp
  * 5237-5393 et al.).  gamma/beta may be NULL. */
@@ -181,6 +185,10 @@ float osb_percentile_key_to_float(unsigned key, int dtype);
 /* NHWC statistics producer for osb_group_norm_apply: stats[2 * groups] += per-group (sum, sum of squares) of y = x + addv[c]; addv and
  * y both null = statistics of x.  cudaErrorInvalidValue for shapes the vector kernel does not cover. */
 int osb_channel_add_stats(const void* x, const void* addv, void* y, int dtype, int64_t C, int64_t HW, int groups, void* stats, void* stream);
+/* Channel Concat of two NHWC images [HW, ca] and [HW, cb] into y [HW, ca + cb], gathering the same per-group statistics of y into `stats` on the
+ * way (the GroupNorm of a UNet up block reads the concatenated skip connection next).  cudaErrorInvalidValue: ca or cb not a multiple of the
+ * 16-byte vector, more than 1024 vectors per pixel or unaligned pointers; nothing is launched then. */
+int osb_concat2_stats(const void* a, const void* b, void* y, int dtype, int64_t ca, int64_t cb, int64_t HW, int groups, void* stats, void* stream);
 int osb_group_norm_apply(const void* x, void* y, int dtype, int64_t C, int64_t HW, int groups, const void* gamma, const void* beta, float eps, int fuse_silu,
                          const void* stats, void* clear_stats, void* stream);
 

@@ -106,6 +106,21 @@ template <typename T> __device__ __forceinline__ T from_float(float v);
 template <> __device__ __forceinline__ float from_float<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half from_float<__half>(float v) { return __float2half_rn(v); }
 
+// ---- binary elementwise arithmetic (OSB_BIN_*), fp32: the node kernels and the tensor-core GEMM's GEGLU epilogue ---------------------
+__device__ __forceinline__ float apply_binary(int op, float a, float b)
+{
+    switch (op) {
+    case OSB_BIN_ADD: return a + b;
+    case OSB_BIN_SUB: return a - b;
+    case OSB_BIN_MUL: return a * b;
+    case OSB_BIN_DIV: return a / b;
+    case OSB_BIN_MUL_GELU: return a * (0.5f * b * (1.f + erff(b * 0.70710678118654752f)));
+    case OSB_BIN_MUL_SIGMOID: return a / (1.f + expf(-b));
+    case OSB_BIN_SILU_MUL: return (a / (1.f + expf(-a))) * b;
+    default: return a;
+    }
+}
+
 // ---- fp32 -> bf16 triple split of the tensor-core fp32 paths (osb_tc_gemm_f32x, osb_flash_attention_f32x) ----------------------------
 // x = h + m + l, h = bf16(x), m = bf16(x - h), l = bf16(x - h - m): 24 mantissa bits in three bf16 planes
 __device__ __forceinline__ void bf16x3_split(float x, __nv_bfloat16& h, __nv_bfloat16& m, __nv_bfloat16& l)

@@ -482,9 +482,10 @@ struct Engine::Impl {
     // ------------------------------------------------------------------------------------------------------
     void exec_step(size_t si);
     void exec_single(size_t oi);
-    void exec_unfused(const Step& s)
+    // the ops of the group from its `done`-th on, one by one (the earlier ones have run)
+    void exec_unfused(const Step& s, size_t done = 0)
     {
-        for (size_t k = 0; k < s.count; k++) exec_single(s.first + k);
+        for (size_t k = done; k < s.count; k++) exec_single(s.first + k);
         if (cur_b + 1 == cur_B)   // intermediates of the group have no consumer outside it: drop them
             for (size_t k = 0; k + 1 < s.count; k++)
                 for (auto& o : E.m_ops[s.first + k].out) if (o.present) {
@@ -1202,6 +1203,14 @@ void Engine::Impl::op_concat(size_t oi)
     }
     Tensor y = make(ty, os, nhwc_path ? Layout::nhwc : Layout::plain);
     y.scale = xs[0].scale; y.zero_point = xs[0].zero_point;
+    if (nhwc_path && xs.size() == 2 && stats_want >= 0 && gn_ring && cur_B == 1 && gn_split_enabled() && gn_apply_ok(y, os[1], stats_groups)) {
+        // the skip-connection Concat of a UNet up block feeding its GroupNorm: one pass copies and gathers the statistics
+        if (osb_concat2_stats(xs[0].data(), xs[1].data(), y.mdata(), K(ty), xs[0].shape[1], xs[1].shape[1], os[2] * os[3], stats_groups, gn_slot_ptr(gn_slot), st) == 0) {
+            stats_ready_for = stats_want;
+            push(oi, 0, y);
+            return;
+        }
+    }
     // physical view: [outer, axis_len * inner]
     int64_t outer = 1, inner = 1, total_axis = os[axis];
     if (nhwc_path) { outer = os[2] * os[3]; inner = 1; }
@@ -2220,32 +2229,59 @@ void Engine::Impl::fused_gelu(const Step& s)
 
 void Engine::Impl::fused_geglu(const Step& s)
 {
-    size_t i = s.first;
-    Tensor x = in(i, 0);
-    auto whole = [&](size_t oi, int64_t lo, int64_t hi) {
+    // a 10-op step starts with the FF-in MatMul + bias Add (plan.cpp: geglu); the gate's 8 ops follow from op i
+    const size_t lead = s.count == 10 ? 2 : 0, i = s.first + lead;
+    // Slice op oi cuts [lo, hi) of the last axis of a rank-`rank` tensor whose last axis has n entries
+    auto cuts = [&](size_t oi, int64_t rank, int64_t n, int64_t lo, int64_t hi) {
         Tensor st_ = in(oi, 1), en = in(oi, 2), ax = in(oi, 3), sp = in(oi, 4);
         if (!st_.i64 || !en.i64 || !ax.i64 || !sp.i64 || st_.i64->size() != 1 || en.i64->size() != 1 || ax.i64->size() != 1 || sp.i64->size() != 1) return false;
-        int64_t a = (*ax.i64)[0], n = x.shape.empty() ? 0 : x.shape.back();
-        if (a < 0) a += (int64_t)x.shape.size();
-        int64_t b = (*st_.i64)[0], e = (*en.i64)[0];
+        int64_t a = (*ax.i64)[0], b = (*st_.i64)[0], e = (*en.i64)[0];
+        if (a < 0) a += rank;
         if (b < 0) b += n;
         if (e < 0) e += n;
-        e = std::min(e, n);
-        return a == (int64_t)x.shape.size() - 1 && (*sp.i64)[0] == 1 && b == lo && e == hi;
+        return a == rank - 1 && (*sp.i64)[0] == 1 && b == lo && std::min(e, n) == hi;
     };
-    int64_t n2 = x.shape.empty() ? 0 : x.shape.back(), inner = n2 / 2;
-    float c0 = scalar_of(in(i + 2, 1), E.m_ops[i + 2]), c1 = scalar_of(in(i + 4, 1), E.m_ops[i + 4]), c2 = scalar_of(in(i + 6, 1), E.m_ops[i + 6]);
-    bool ok = (x.type == DType::f16 || x.type == DType::f32) && x.layout == Layout::plain && n2 >= 2 && n2 % 2 == 0 &&
-              whole(i, 0, inner) && whole(i + 1, inner, n2) && std::fabs(c0 - 1.41421356f) <= 1e-3f && c1 == 1.f && c2 == 0.5f;
-    if (!ok) {
+    // the halves of a rank-`rank` [.., n] tensor, and the constants of the erf GELU
+    auto gate_ok = [&](int64_t rank, int64_t n) {
+        float c0 = scalar_of(in(i + 2, 1), E.m_ops[i + 2]), c1 = scalar_of(in(i + 4, 1), E.m_ops[i + 4]), c2 = scalar_of(in(i + 6, 1), E.m_ops[i + 6]);
+        return n >= 2 && n % 2 == 0 && cuts(i, rank, n, 0, n / 2) && cuts(i + 1, rank, n, n / 2, n) && std::fabs(c0 - 1.41421356f) <= 1e-3f && c1 == 1.f && c2 == 0.5f;
+    };
+    if (lead) {
+        const size_t mm = s.first;
+        Tensor a = to_plain(in(mm, 0)), bias = in(mm + 1, (size_t)s.bias_in);
+        const TensorRef& wr = E.m_ops[mm].in[1];
+        const int64_t Kd = wr.shape[0], inner = wr.shape[1] / 2, M = !a.shape.empty() && a.shape.back() == Kd && Kd > 0 ? a.numel() / Kd : 0;
+        if (a.type == DType::f16 && E.gemm_impl != 1 && M > 0 && gate_ok((int64_t)a.shape.size(), wr.shape[1])) {
+            Tensor w = in(mm, 1);
+            if (w.type != a.type) w = convert(w, a.type);
+            if (bias.type != a.type) bias = convert(bias, a.type);
+            std::vector<int64_t> os = a.shape; os.back() = inner;
+            Tensor y = make(a.type, os);
+            const int rc = osb_tc_gemm_geglu(a.data(), w.data(), y.mdata(), bias.data(), M, inner, Kd, st);
+            if (rc != (int)cudaErrorNotSupported) {
+                ck(rc, "osb_tc_gemm_geglu");
+                push(i + 7, 0, y);
+                return;
+            }
+        }
+        op_matmul(mm, &bias, nullptr, mm + 1);     // the unfused chain: the bias GEMM, then the gate pass below
+    }
+    Tensor x = in(i, 0);
+    const int64_t n2 = x.shape.empty() ? 0 : x.shape.back(), inner = n2 / 2;
+    if (!((x.type == DType::f16 || x.type == DType::f32) && x.layout == Layout::plain && gate_ok((int64_t)x.shape.size(), n2))) {
         // not the two halves (or an unexpected constant): run the group with the ordinary handlers
-        exec_unfused(s);
+        exec_unfused(s, lead);
         return;
     }
     std::vector<int64_t> os = x.shape; os.back() = inner;
     Tensor y = make(x.type, os);
     ck(osb_geglu(x.data(), y.mdata(), K(x.type), x.numel() / n2, inner, st), "osb_geglu");
     push(i + 7, 0, y);
+    if (lead && cur_b + 1 == cur_B) {   // the GEMM's [.., 2 inner] result has no consumer outside the step
+        const std::string& xn = E.m_ops[s.first + 1].out[0].name;
+        store.erase(xn);
+        order.erase(std::remove(order.begin(), order.end(), xn), order.end());
+    }
 }
 
 void Engine::Impl::fused_silu(const Step& s)

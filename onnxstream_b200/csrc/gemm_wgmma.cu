@@ -85,6 +85,7 @@ struct TcParams {
     long long stride_c;          // elements between batches
     long long ldc;               // elements between output rows (== N for a dense C)
     int bm, bn;                  // the tile shape the launch runs (the kernel's template arguments; kept for the launch profile)
+    int geglu;                   // GEGLU epilogue (osb_tc_gemm_geglu): B is [K, 2 N], C [M, N] = value * gelu(gate)
 };
 
 using namespace tcptx;
@@ -120,8 +121,10 @@ __device__ __forceinline__ __half2 ld_pair(const __half* x, bool ok0, bool ok1, 
 // BM x BN = the tile (TileCfg).  EXTRAS = the epilogue also adds `bias2` and gathers GroupNorm statistics.  A separate instantiation, so
 // the common launches do not carry the extra registers and code.  B_MN_MAJOR (== !p.b_kmajor) and BF16 (== p.bf16) are compile-time: the
 // MMA loop has no branches.  PAIR = launched as clusters of two CTAs (see the top of the file); 128 x 128 tiles, split_k == 1 and
-// groups == 1 there.
-template <int BM, int BN, bool EXTRAS, int B_MN_MAJOR, bool BF16, bool PAIR>
+// groups == 1 there.  GEGLU (== p.geglu; 128 x 128 tiles, MN-major B, split_k == 1): the feed-forward gate of a [K, 2 N] weight in the
+// epilogue.  The tile's B atom 0 holds value columns [64 nt, 64 nt + 64), atom 1 the gate columns N + [64 nt, 64 nt + 64), so every thread
+// holds value block j and its gate block j + 8 in the same rows and column pair; the tile stores 64 columns of C [M, N].
+template <int BM, int BN, bool EXTRAS, int B_MN_MAJOR, bool BF16, bool PAIR, bool GEGLU = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_b1,
                const __grid_constant__ CUtensorMap map_b2, const TcParams p)
@@ -130,6 +133,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     constexpr int STAGES = Cfg::STAGES, A_STAGE_BYTES = Cfg::A_STAGE_BYTES, B_STAGE_BYTES = Cfg::B_STAGE_BYTES, WN = Cfg::WN;
     static_assert(!PAIR || (BM == 128 && BN == 128), "CTA pairs run 128 x 128 tiles");
     static_assert(!B_MN_MAJOR || WN % 64 == 0, "an MN-major B is read in 64-column atoms");
+    static_assert(!GEGLU || (BM == 128 && BN == 128 && B_MN_MAJOR && !EXTRAS && !BF16 && !PAIR), "GEGLU: 128 x 128 tiles of an fp16 [K, 2 N] weight");
     osb_pdl_trigger_entry();   // let the next kernel's CTAs be scheduled as ours drain; it waits for our completion before touching memory
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment for the 128B swizzle atoms
@@ -218,8 +222,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         // BN/64 atoms of 64 columns x 64 k-rows
 #pragma unroll
                         for (int at = 0; at < BN / 64; at++) {
-                            if (p.b_swap) tma_load_3d_s(sb + at * 8192, mbp, &full[stage], n0 + 64 * at, b, kglob);
-                            else tma_load_3d_s(sb + at * 8192, mbp, &full[stage], n0 + 64 * at, kglob, b);
+                            const int col = GEGLU ? 64 * nt + at * p.N : n0 + 64 * at;     // GEGLU: the value atom, then the gate atom
+                            if (p.b_swap) tma_load_3d_s(sb + at * 8192, mbp, &full[stage], col, b, kglob);
+                            else tma_load_3d_s(sb + at * 8192, mbp, &full[stage], col, kglob, b);
                         }
                     }
                 }
@@ -319,6 +324,28 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             release(prev);
 
             // ---- epilogue ----
+            if constexpr (GEGLU) {
+                // each half rounded to fp16 as the plain bias epilogue stores it, then value * gelu(gate) in fp32 (the node kernel's
+                // arithmetic), rounded once: bit-identical to the unsplit GEMM followed by osb_geglu
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                    const int n = 64 * nt + 8 * j + cq;      // value column; the gate is column p.N + n
+                    float av0 = 0.f, av1 = 0.f, ag0 = 0.f, ag1 = 0.f;
+                    if (p.bias) {
+                        const __half2 bv = ld_pair<true>(p.bias + n, true, true, vec_bias), bg = ld_pair<true>(p.bias + p.N + n, true, true, vec_bias);
+                        av0 += __low2float(bv); av1 += __high2float(bv); ag0 += __low2float(bg); ag1 += __high2float(bg);
+                    }
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        if (!row_ok[h]) continue;
+                        const float a0 = __half2float(__float2half_rn(acc[4 * j + 2 * h] + av0)), a1 = __half2float(__float2half_rn(acc[4 * j + 2 * h + 1] + av1));
+                        const float g0 = __half2float(__float2half_rn(acc[4 * (j + 8) + 2 * h] + ag0)), g1 = __half2float(__float2half_rn(acc[4 * (j + 8) + 2 * h + 1] + ag1));
+                        *reinterpret_cast<__half2*>(p.C + off[h] + n) =
+                            __halves2half2(__float2half_rn(apply_binary(OSB_BIN_MUL_GELU, a0, g0)), __float2half_rn(apply_binary(OSB_BIN_MUL_GELU, a1, g1)));
+                    }
+                }
+                continue;
+            }
             __half* cbase = p.C;
             if (p.groups > 1) cbase = b == 0 ? p.C : (b == 1 ? p.C1 : p.C2);    // stride_c == 0 in a grouped launch
             const bool pair_ok = (p.N & 1) == 0 && (p.ldc & 1) == 0;           // two adjacent columns move as one 4- / 8-byte vector
@@ -629,12 +656,12 @@ void prof_begin(ProfRec& rec, const TcParams& p, cudaStream_t st)
     cudaEventCreate(&rec.a); cudaEventCreate(&rec.b);
     // the fp32 path (bf16 triple split) runs a 6x longer K: ALGORITHMIC work is the fp32 problem's (K / 6, 4-byte elements)
     const double kdiv = p.bf16 ? 6.0 : 1.0, es = p.bf16 ? 4.0 : 2.0;
-    double M = p.M, N = p.N, Kt = (double)p.K * p.taps / kdiv, B = p.batch;
+    double M = p.M, N = p.geglu ? 2.0 * p.N : p.N, Kt = (double)p.K * p.taps / kdiv, B = p.batch;
     rec.flops = 2.0 * M * N * Kt * B;
     // algorithmic bytes: A once (conv: the input image once), B once, C once (+ residual / bias reads)
     double a_bytes = (p.bh > 0 ? M * (p.K / kdiv) : M * Kt) * es * B;
-    rec.bytes = a_bytes + N * Kt * es * (p.bh > 0 ? 1.0 : B) + M * N * es * B * (p.residual ? 2.0 : 1.0) + (p.bias ? N * es : 0.0);
-    rec.M = p.M; rec.N = p.N; rec.K = p.K; rec.taps = p.taps; rec.batch = p.batch; rec.split = p.split_k; rec.conv = p.bh > 0;
+    rec.bytes = a_bytes + N * Kt * es * (p.bh > 0 ? 1.0 : B) + M * p.N * es * B * (p.residual ? 2.0 : 1.0) + (p.bias ? N * es : 0.0);
+    rec.M = p.M; rec.N = (int)N; rec.K = p.K; rec.taps = p.taps; rec.batch = p.batch; rec.split = p.split_k; rec.conv = p.bh > 0;
     rec.bm = p.bm; rec.bn = p.bn; rec.kmajor = p.b_kmajor;
     cudaEventRecord(rec.a, st);
 }
@@ -642,13 +669,13 @@ void prof_begin(ProfRec& rec, const TcParams& p, cudaStream_t st)
 using TcKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TcParams);
 
 // the instantiation, with its shared-memory limit raised once
-template <int BM, int BN, bool EXTRAS, int B_MN_MAJOR, bool BF16, bool PAIR>
+template <int BM, int BN, bool EXTRAS, int B_MN_MAJOR, bool BF16, bool PAIR, bool GEGLU = false>
 TcKernel ready_kernel(int* err)
 {
-    static const cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<BM, BN, EXTRAS, B_MN_MAJOR, BF16, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    static const cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<BM, BN, EXTRAS, B_MN_MAJOR, BF16, PAIR, GEGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                       TileCfg<BM, BN>::SMEM_BYTES);
     *err = (int)e;
-    return tc_gemm_kernel<BM, BN, EXTRAS, B_MN_MAJOR, BF16, PAIR>;
+    return tc_gemm_kernel<BM, BN, EXTRAS, B_MN_MAJOR, BF16, PAIR, GEGLU>;
 }
 
 // the kernel for a launch; nullptr when (bm, bn) is not instantiated for its B layout / epilogue / type
@@ -660,6 +687,10 @@ TcKernel pick_kernel(const TcParams& p, bool extras, bool pair, int* smem, int* 
         if (p.bf16 || p.split_k != 1 || p.groups > 1 || p.bm != 128 || p.bn != 128) return nullptr;
         return extras ? (p.b_kmajor ? ready_kernel<128, 128, true, 0, false, true>(err) : ready_kernel<128, 128, true, 1, false, true>(err))
                       : (p.b_kmajor ? ready_kernel<128, 128, false, 0, false, true>(err) : ready_kernel<128, 128, false, 1, false, true>(err));
+    }
+    if (p.geglu) {
+        if (extras || p.bf16 || p.b_kmajor || p.split_k != 1 || p.groups > 1 || p.bm != 128 || p.bn != 128) return nullptr;
+        return ready_kernel<128, 128, false, 1, false, false, true>(err);
     }
     if (p.bf16) {   // the fp32 path: no bias2 / statistics
         if (p.bm != 128 || p.bn != 128) return nullptr;
@@ -1018,6 +1049,29 @@ int osb_tc_gemm_grouped_launch(const void* A, const void* const* B, void* const*
     p.bias = nullptr; p.residual = nullptr; p.stride_c = 0; p.ldc = ldc;
     p.split_k = 1; p.ws = nullptr;
     return launch(ma, mb[0], p, st, &mb[1], groups > 2 ? &mb[2] : &mb[1]);
+}
+
+// The GEGLU feed-forward gate in the GEMM epilogue: C [M, inner] = value * gelu_erf(gate) of (A [M, K] . B [K, 2 inner] + bias [2 inner]),
+// one unsplit launch of 128 x 128 tiles (64 value + 64 gate columns each), fp16, dense operands.  Measured faster than the rule's GEMM plus
+// the GEGLU pass at every SD 1.5 feed-forward shape, the 8x8 level's (M = 64, where the rule's pick is a 64 x 128 tile) included (DESIGN.md
+// section 5), so it has no rule of its own.
+extern "C" int osb_tc_gemm_geglu(const void* A, const void* B, void* C, const void* bias, int64_t M, int64_t inner, int64_t K, void* stream)
+{
+    if (inner < 64 || inner % 64 || !osb_tc_gemm_ok(M, 2 * inner, K, 0, A, B, C, 0, 0, 0, K, 2 * inner, inner) || ((uintptr_t)bias & 3)) return (int)cudaErrorNotSupported;
+    CUtensorMap ma, mb;
+    int a_swap = 0, b_swap = 0;
+    if (!make_map_rb(&ma, A, (uint64_t)K, (uint64_t)M, 1, (uint64_t)K * 2, (uint64_t)(M * K) * 2, BLOCK_K, BLOCK_M, &a_swap)) return (int)cudaErrorInvalidValue;
+    if (!make_map_rb(&mb, B, (uint64_t)(2 * inner), (uint64_t)K, 1, (uint64_t)(2 * inner) * 2, (uint64_t)(2 * inner * K) * 2, 64, BLOCK_K, &b_swap))
+        return (int)cudaErrorInvalidValue;
+    TcParams p{};
+    p.M = (int)M; p.N = (int)inner; p.K = (int)K; p.batch = 1;
+    p.bm = BLOCK_M; p.bn = BLOCK_N; p.geglu = 1;
+    p.m_tiles = (int)((M + BLOCK_M - 1) / BLOCK_M); p.n_tiles = (int)(inner / 64);
+    p.taps = 1; p.kw = 1; p.tiles_x = 1; p.stride = 1;
+    p.k_blocks_per_tap = (int)((K + BLOCK_K - 1) / BLOCK_K);
+    p.C = (__half*)C; p.bias = (const __half*)bias; p.ldc = inner;
+    p.split_k = 1;
+    return launch(ma, mb, p, (cudaStream_t)stream);
 }
 
 bool osb_tc_conv_ok(int64_t H, int64_t W, int64_t Cin, int64_t Cout, int kh, int kw, int stride, const void* x, const void* w, const void* y)

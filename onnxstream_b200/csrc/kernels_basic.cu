@@ -98,20 +98,6 @@ __global__ void unary_kernel(int op, const T* __restrict__ x, T* __restrict__ y,
 // binary with broadcasting
 // ------------------------------------------------------------------------------------------------------------
 
-__device__ __forceinline__ float apply_binary(int op, float a, float b)
-{
-    switch (op) {
-    case OSB_BIN_ADD: return a + b;
-    case OSB_BIN_SUB: return a - b;
-    case OSB_BIN_MUL: return a * b;
-    case OSB_BIN_DIV: return a / b;
-    case OSB_BIN_MUL_GELU: return a * (0.5f * b * (1.f + erff(b * 0.70710678118654752f)));
-    case OSB_BIN_MUL_SIGMOID: return a / (1.f + expf(-b));
-    case OSB_BIN_SILU_MUL: return (a / (1.f + expf(-a))) * b;
-    default: return a;
-    }
-}
-
 struct BinParams {
     int64_t shape[OSB_MAX_DIMS];
     int64_t as[OSB_MAX_DIMS];
@@ -522,11 +508,12 @@ __global__ void gn_stats_nhwc_kernel(const T* __restrict__ x, double* __restrict
     for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) atomicAdd(&stats[i], (double)sm[i]);
 }
 
-// y's value at pixel 0, channel c (y = x, or x + addv[c] rounded to T): the pivot of the group that starts at channel c, which
-// every CTA computes alike
-template <typename T>
-__device__ __forceinline__ float gn_first_y(const T* __restrict__ x, const T* __restrict__ addv, int c)
+// y's value at pixel 0, channel c (y = x, x + addv[c] rounded to T, or channel c of the concatenation [x | xb] with ca channels from x):
+// the pivot of the group that starts at channel c, which every CTA computes alike
+template <typename T, bool CAT>
+__device__ __forceinline__ float gn_first_y(const T* __restrict__ x, const T* __restrict__ addv, int c, const T* __restrict__ xb, int ca)
 {
+    if (CAT) return to_float(c < ca ? x[c] : xb[c - ca]);
     const float v = to_float(x[c]);
     return addv ? to_float(from_float<T>(v + to_float(addv[c]))) : v;
 }
@@ -534,10 +521,12 @@ __device__ __forceinline__ float gn_first_y(const T* __restrict__ x, const T* __
 // NHWC statistics, vectorised: a thread owns 8 consecutive channels (one 16-byte load per pixel) and walks down the
 // CTA's pixel strip; 256/(C/8) pixels are in flight per iteration.  Per-channel fp32 partials of y - p (p: the group's pivot,
 // gn_first_y) go to shared memory, are folded per group in fp64, then one double atomic per bin and CTA.
-template <typename T, int VEC>
+template <typename T, int VEC, bool CAT = false>
 __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __restrict__ stats, int C, int64_t HW, int groups, int64_t pix_per_cta,
-                                         const T* __restrict__ addv = nullptr, T* __restrict__ y = nullptr, int pivot = 0)
+                                         const T* __restrict__ addv, T* __restrict__ y, int pivot, const T* __restrict__ xb, int ca)
 {
+    // CAT: y = the channel concatenation of x [HW, ca] and xb [HW, C - ca] (ca % VEC == 0: a thread's channels come from one source),
+    // copied on the way; the statistics are those of y as for the Add.
     // addv / y != null: y = x + addv[c] (the per-channel time-embedding add of a resnet) is written on the way and the statistics
     // are those of y -- the producer side of a GroupNorm whose apply pass is gn_apply_pre_kernel.  pivot != 0: the sums of y - p
     // go out as they are (osb_group_norm's layout, see gn_mean_var); else they are shifted back to plain sums of y and y^2, which
@@ -545,11 +534,15 @@ __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __rest
     // sums of y and y^2 would cancel in E[y^2] - mean^2 when the mean is large against the spread.
     osb_pdl_prologue();
     extern __shared__ float sm[];  // the group pivots (groups of the 2 * groups floats), then the per-row partials
-    for (int g = threadIdx.x; g < groups; g += blockDim.x) sm[g] = gn_first_y(x, addv, g * (C / groups));
+    for (int g = threadIdx.x; g < groups; g += blockDim.x) sm[g] = gn_first_y<T, CAT>(x, addv, g * (C / groups), xb, ca);
     __syncthreads();
     const int tpp = C / VEC;                        // threads per pixel
     const int rows = blockDim.x / tpp;              // pixels in flight
     const int cv = threadIdx.x % tpp, pr = threadIdx.x / tpp;
+    // where this thread's channels are read: x + pixel * C, or (CAT) its source's channel offset and pixel stride
+    const T* src = x + cv * VEC;
+    int64_t src_ld = C;
+    if (CAT) { if (cv * VEC < ca) src_ld = ca; else { src = xb + (cv * VEC - ca); src_ld = C - ca; } }
     int64_t p0 = (int64_t)blockIdx.x * pix_per_cta, p1 = min(p0 + pix_per_cta, HW);
     const int cpg = C / groups;
     if (pr < rows) {
@@ -565,14 +558,16 @@ __global__ void gn_stats_nhwc_vec_kernel(const T* __restrict__ x, double* __rest
         for (int64_t pb = p0 + pr; pb < p1; pb += 4 * (int64_t)rows) {
             Vec<T, VEC> v[4];
 #pragma unroll
-            for (int u = 0; u < 4; u++) { const int64_t p = pb + u * (int64_t)rows; if (p < p1) v[u] = load_vec<T, VEC>(x + p * C + cv * VEC); }
+            for (int u = 0; u < 4; u++) { const int64_t p = pb + u * (int64_t)rows; if (p < p1) v[u] = load_vec<T, VEC>(src + p * src_ld); }
 #pragma unroll
             for (int u = 0; u < 4; u++) {
                 const int64_t p = pb + u * (int64_t)rows;
                 if (p >= p1) break;
                 if (y) {
+                    if (!CAT) {
 #pragma unroll
-                    for (int k = 0; k < VEC; k++) v[u].v[k] = from_float<T>(to_float(v[u].v[k]) + a[k]);
+                        for (int k = 0; k < VEC; k++) v[u].v[k] = from_float<T>(to_float(v[u].v[k]) + a[k]);
+                    }
                     store_vec<T, VEC>(y + p * C + cv * VEC, v[u]);
                 }
 #pragma unroll
@@ -1412,8 +1407,8 @@ int osb_group_norm(const void* x, void* y, int dtype, int nhwc, int64_t C, int64
             int64_t ppc2 = (HW + c2 - 1) / c2;
             c2 = (HW + ppc2 - 1) / ppc2;
             const size_t smem2 = sizeof(float) * (2 * groups + (size_t)(256 / (C / vec)) * 2 * C);    // + the per-row partials
-            if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8>), (unsigned)c2, 256, smem2, st, (const __half*)x, stats, (int)C, HW, groups, ppc2, (const __half*)nullptr, (__half*)nullptr, 1);
-            else if (dtype == OSB_F32) osb_launch((gn_stats_nhwc_vec_kernel<float, 4>), (unsigned)c2, 256, smem2, st, (const float*)x, stats, (int)C, HW, groups, ppc2, (const float*)nullptr, (float*)nullptr, 1);
+            if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8>), (unsigned)c2, 256, smem2, st, (const __half*)x, stats, (int)C, HW, groups, ppc2, (const __half*)nullptr, (__half*)nullptr, 1, (const __half*)nullptr, 0);
+            else if (dtype == OSB_F32) osb_launch((gn_stats_nhwc_vec_kernel<float, 4>), (unsigned)c2, 256, smem2, st, (const float*)x, stats, (int)C, HW, groups, ppc2, (const float*)nullptr, (float*)nullptr, 1, (const float*)nullptr, 0);
             else return (int)cudaErrorInvalidValue;
             goto stats_done;
         }
@@ -1481,8 +1476,32 @@ int osb_channel_add_stats(const void* x, const void* addv, void* y, int dtype, i
     int64_t ppc2 = (HW + c2 - 1) / c2;
     c2 = (HW + ppc2 - 1) / ppc2;
     size_t smem = sizeof(float) * (2 * groups + (size_t)rows_per_cta * 2 * C);
-    if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8>), (unsigned)c2, 256, smem, st, (const __half*)x, (double*)stats, (int)C, HW, groups, ppc2, (const __half*)addv, (__half*)y, 0);
-    else osb_launch((gn_stats_nhwc_vec_kernel<float, 4>), (unsigned)c2, 256, smem, st, (const float*)x, (double*)stats, (int)C, HW, groups, ppc2, (const float*)addv, (float*)y, 0);
+    if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8>), (unsigned)c2, 256, smem, st, (const __half*)x, (double*)stats, (int)C, HW, groups, ppc2, (const __half*)addv, (__half*)y, 0, (const __half*)nullptr, 0);
+    else osb_launch((gn_stats_nhwc_vec_kernel<float, 4>), (unsigned)c2, 256, smem, st, (const float*)x, (double*)stats, (int)C, HW, groups, ppc2, (const float*)addv, (float*)y, 0, (const float*)nullptr, 0);
+    return launched();
+}
+
+// Channel Concat of two NHWC images that a GroupNorm reads next: y [HW, ca + cb] = [a | b] in one pass that also adds the per-group (sum, sum
+// of squares) of y to stats[2 * groups], as osb_channel_add_stats does for the Add.  cudaErrorInvalidValue: a layout the kernel does not cover
+// (a source's channels not a multiple of the vector, more than 1024 vectors per pixel, unaligned pointers); nothing is launched then.
+int osb_concat2_stats(const void* a, const void* b, void* y, int dtype, int64_t ca, int64_t cb, int64_t HW, int groups, void* stats, void* stream)
+{
+    const int vec = dtype == OSB_F16 ? 8 : 4;
+    const int64_t C = ca + cb;
+    if ((dtype != OSB_F16 && dtype != OSB_F32) || HW < 1 || groups < 1 || ca < 1 || cb < 1 || C % groups || ca % vec || cb % vec || C / vec > 1024 ||
+        !aligned16(a) || !aligned16(b) || !aligned16(y))
+        return (int)cudaErrorInvalidValue;
+    // one pixel's vectors per thread row, as many rows as fit 256 threads (a wider pixel takes a block of its own width)
+    const int tpp = (int)(C / vec), threads = tpp <= 256 ? 256 : (tpp + 31) / 32 * 32, rows_per_cta = threads / tpp;
+    int64_t c2 = max<int64_t>(1, min<int64_t>((HW + 4 * rows_per_cta - 1) / (4 * rows_per_cta), OSB_SMS * 4));
+    const int64_t ppc2 = (HW + c2 - 1) / c2;
+    c2 = (HW + ppc2 - 1) / ppc2;
+    const size_t smem = sizeof(float) * (2 * groups + (size_t)rows_per_cta * 2 * C);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == OSB_F16) osb_launch((gn_stats_nhwc_vec_kernel<__half, 8, true>), (unsigned)c2, threads, smem, st, (const __half*)a, (double*)stats, (int)C, HW, groups, ppc2,
+                                     (const __half*)nullptr, (__half*)y, 0, (const __half*)b, (int)ca);
+    else osb_launch((gn_stats_nhwc_vec_kernel<float, 4, true>), (unsigned)c2, threads, smem, st, (const float*)a, (double*)stats, (int)C, HW, groups, ppc2,
+                    (const float*)nullptr, (float*)y, 0, (const float*)b, (int)ca);
     return launched();
 }
 

@@ -196,9 +196,18 @@ struct Planner {
 
     // GEGLU gate: Slice(x, 0:inner), Slice(x, inner:2*inner) on the last axis, gelu_erf of the second, Mul -- one kernel, no
     // materialised halves.  The slice bounds are int64 weights, so they are verified when the step executes (fused_geglu falls
-    // back to the op-by-op path if they are not the two halves).
+    // back to the op-by-op path if they are not the two halves).  Led by MatMul(x, W[K, 2 inner]) -> Add(bias) whose result only the
+    // two Slices read, the step takes those too (10 ops): the gate runs in the GEMM epilogue where fused_geglu can launch it so.
     size_t geglu(size_t i, Step& s) const
     {
+        if (types_at(i, { "MatMul", "Add" })) {
+            Step lin;
+            if (linear(i, lin) != 2 || lin.bias_in < 0 || upcast(ops[i])) return 0;
+            const std::string& x = ops[i + 1].out[0].name;
+            if (!used(x, 2) || geglu(i + 2, s) != 8 || ops[i + 2].in[0].name != x) return 0;
+            s.bias_in = lin.bias_in;
+            return 10;
+        }
         if (!types_at(i, { "Slice", "Slice" })) return 0;
         const OpDef &s0 = ops[i], &s1 = ops[i + 1];
         if (s0.in.size() != 5 || s1.in.size() != 5 || s0.out.size() != 1 || s1.out.size() != 1) return 0;
@@ -474,7 +483,7 @@ Plan make_plan(const std::vector<OpDef>& ops, const PlanOptions& o)
         i += s.count;
     }
     const auto& steps = p.steps;
-    // GroupNorm steps whose input is produced by the step right before them (conv / conv + residual / per-channel Add): that
+    // GroupNorm steps whose input is produced by the step right before them (conv / conv + residual / per-channel Add / Concat): that
     // producer gathers the statistics (fuse_nodes only; the op list is unchanged, only the GroupNorm's stats pass disappears)
     p.stats_consumer.assign(steps.size(), -1);
     for (size_t j = 1; j < steps.size(); j++) {
@@ -482,7 +491,7 @@ Plan make_plan(const std::vector<OpDef>& ops, const PlanOptions& o)
         const Step& pstep = steps[j - 1];
         const OpDef& last = ops[pstep.first + pstep.count - 1];
         if (last.out.size() != 1 || last.out[0].name != ops[steps[j].first].in[0].name) continue;
-        if (pstep.kind == SK_CONV_ADD || (pstep.kind == SK_SINGLE && (last.type == "Conv" || last.type == "Add"))) p.stats_consumer[j - 1] = (long)j;
+        if (pstep.kind == SK_CONV_ADD || (pstep.kind == SK_SINGLE && (last.type == "Conv" || last.type == "Add" || last.type == "Concat"))) p.stats_consumer[j - 1] = (long)j;
     }
     p.step_weights.assign(steps.size(), {});
     for (size_t si = 0; si < steps.size(); si++) {
