@@ -202,6 +202,17 @@ struct Engine::Impl {
 
     bool upcast_op(const OpDef& op) const { return runs_upcast(op, E.use_fp16_arithmetic, E.requires_upcast); }
 
+    // fp32 arithmetic meeting an fp16 blob on a decode-shaped MatMul (activation rows <= 8 times a static 2-D weight, plan.cpp
+    // is_gemv_matmul): the GEMV reads the weight as stored and widens it in registers, the same fp32 operand the load-time conversion
+    // (src/onnxstream.cpp:2892-2900) would have made, at half the bytes
+    bool f16w_gemv(const OpDef& op, const Tensor& a) const
+    {
+        const TensorRef& wr = op.in[1];
+        if (a.type != DType::f32 || E.use_fp16_arithmetic || wr.wtype != DType::f16 || wr.shape.size() != 2 || a.shape.empty() || a.shape.back() != wr.shape[0] || upcast_op(op)) return false;
+        int64_t rows = 1; for (size_t k = 0; k + 1 < a.shape.size(); k++) rows *= a.shape[k];
+        return rows <= 8;
+    }
+
     DType act_dtype() const { return E.use_fp16_arithmetic ? DType::f16 : DType::f32; }
 
     // ------------------------------------------------------------------------------------------------------
@@ -276,7 +287,8 @@ struct Engine::Impl {
         }
     }
 
-    Tensor get_weight(size_t op_idx, size_t in_idx, bool requires_float = false, bool conv_layout = false, bool keep_u8 = false)
+    // keep_stored: a uint8 or fp16 blob stays as stored -- the consumer dequantises / widens it in registers (decode GEMV): no float copy in HBM
+    Tensor get_weight(size_t op_idx, size_t in_idx, bool requires_float = false, bool conv_layout = false, bool keep_stored = false)
     {
         const OpDef& op = E.m_ops[op_idx];
         const TensorRef& r = op.in[in_idx];
@@ -285,7 +297,7 @@ struct Engine::Impl {
         if (conv_w && !conv_layout) throw std::invalid_argument("Model::get_tensor_data: nchw layout not supported. (not implemented)");
         if (!conv_w && conv_layout) throw std::invalid_argument("Model::get_tensor_data: unable to determine tensor data file compatible with required_layout.");
         DType target = weight_target(op, r, requires_float);
-        if (keep_u8 && r.wtype == DType::u8) target = DType::u8;     // the consumer dequantises in registers (decode GEMV): no float copy in HBM
+        if (keep_stored && (r.wtype == DType::u8 || r.wtype == DType::f16)) target = r.wtype;
 
         Tensor t;
         t.name = fn;
@@ -354,6 +366,26 @@ struct Engine::Impl {
         }
         if (E.resident_weights) { resident[rkey] = t; resident_bytes += (size_t)numel * dtype_size(target); }
         return t;
+    }
+
+    // The resident weight `name` ([Kd][N], b) as a row-padded copy [Kd][Np], Np = N rounded up to the 16-byte vector, zero in the pad:
+    // made once and kept with the resident weights, it lets the vector GEMV stream a weight whose rows are not 16-byte granular (a
+    // 32003-entry vocabulary; the scalar kernel ran at a fifth of the rate)
+    Tensor padded_weight(const std::string& name, const Tensor& b, int64_t Kd, int64_t N)
+    {
+        const size_t es = dtype_size(b.type);
+        const int64_t vec = 16 / (int64_t)es, Np = (N + vec - 1) / vec * vec;
+        const std::string pkey = name + "|pad" + std::to_string((int)b.type);
+        auto it = resident.find(pkey);
+        if (it == resident.end()) {
+            Tensor bp = make(b.type, { Kd, Np });
+            ck(cudaMemsetAsync(bp.mdata(), 0, (size_t)(Kd * Np) * es, st), "cudaMemsetAsync(padded weight)");
+            ck(cudaMemcpy2DAsync(bp.mdata(), (size_t)Np * es, b.data(), (size_t)N * es, (size_t)N * es, (size_t)Kd, cudaMemcpyDeviceToDevice, st),
+               "cudaMemcpy2DAsync(padded weight)");
+            resident_bytes += (size_t)(Kd * Np) * es;
+            it = resident.emplace(pkey, bp).first;
+        }
+        return it->second;
     }
 
     // ------------------------------------------------------------------------------------------------------
@@ -837,6 +869,25 @@ void Engine::Impl::op_matmul(size_t oi, const Tensor* bias, const Tensor* residu
             }
         }
     }
+    if (f16w_gemv(op, a)) {
+        const TensorRef& wr = op.in[1];
+        const int64_t Kd = wr.shape[0], N = wr.shape[1];
+        int64_t rows = 1; for (size_t k = 0; k + 1 < a.shape.size(); k++) rows *= a.shape[k];
+        Tensor w = get_weight(oi, 1, false, false, true);
+        int64_t ldb = N;
+        if (E.resident_weights && N % 8 != 0 && N >= 256 && Kd >= 64) { w = padded_weight(wr.name, w, Kd, N); ldb = w.shape[1]; }
+        Tensor bb, rr;
+        if (bias) { bb = *bias; if (bb.type != a.type) bb = convert(bb, a.type); }
+        if (residual) { rr = to_plain(*residual); if (rr.type != a.type) rr = convert(rr, a.type); }
+        std::vector<int64_t> os = a.shape; os.back() = N;
+        Tensor y = make(a.type, os);
+        const int rc = osb_gemv_f16w(a.data(), w.data(), ldb, y.mdata(), bias ? bb.data() : nullptr, residual ? rr.data() : nullptr, rows, N, Kd, st);
+        if (rc == 0) {
+            push(out_op == (size_t)-1 ? oi : out_op, 0, y);
+            return;
+        }
+        if (rc != (int)cudaErrorNotSupported) ck(rc, "osb_gemv_f16w");
+    }
     Tensor b = to_plain(in(oi, 1));
     std::vector<int64_t> as = a.shape, bs = b.shape;
     bool lead1 = false, first2d = false;
@@ -892,20 +943,9 @@ void Engine::Impl::op_matmul(size_t oi, const Tensor* bias, const Tensor* residu
         }
         const int64_t vec = 16 / (int64_t)dtype_size(a.type);
         if (E.resident_weights && op.in[1].wtype != DType::none && op.in[1].shape.size() == 2 && n == 1 && M <= 8 && N >= 256 && N % vec != 0 && Kd >= 64) {
-            // decode GEMV against a resident weight whose rows are not 16-byte granular (a 32003-entry vocabulary): a row-padded copy,
-            // made once and kept with the resident weights, lets the vector GEMV stream it (the scalar kernel ran at a fifth of the rate)
-            const int64_t Np = (N + vec - 1) / vec * vec;
-            const std::string pkey = op.in[1].name + "|pad" + std::to_string((int)a.type);
-            auto it = resident.find(pkey);
-            if (it == resident.end()) {
-                Tensor bp = make(a.type, { Kd, Np });
-                ck(cudaMemsetAsync(bp.mdata(), 0, (size_t)(Kd * Np) * dtype_size(a.type), st), "cudaMemsetAsync(padded weight)");
-                ck(cudaMemcpy2DAsync(bp.mdata(), (size_t)Np * dtype_size(a.type), b.data(), (size_t)N * dtype_size(a.type), (size_t)N * dtype_size(a.type), (size_t)Kd,
-                                     cudaMemcpyDeviceToDevice, st), "cudaMemcpy2DAsync(padded weight)");
-                resident_bytes += (size_t)(Kd * Np) * dtype_size(a.type);
-                it = resident.emplace(pkey, bp).first;
-            }
-            ck(osb_gemm_ld(a.data(), Kd, it->second.data(), Np, y.mdata(), N, bias ? bb.data() : nullptr, residual ? rr.data() : nullptr, 1, M, N, Kd,
+            // decode GEMV against a resident weight whose rows are not 16-byte granular (a 32003-entry vocabulary): see padded_weight
+            const Tensor bp = padded_weight(op.in[1].name, b, Kd, N);
+            ck(osb_gemm_ld(a.data(), Kd, bp.data(), bp.shape[1], y.mdata(), N, bias ? bb.data() : nullptr, residual ? rr.data() : nullptr, 1, M, N, Kd,
                            0, 0, 0, 0, K(a.type), E.gemm_impl, st), "osb_gemm_ld(padded weight)");
         } else
         ck(osb_gemm(a.data(), b.data(), y.mdata(), bias ? bb.data() : nullptr, residual ? rr.data() : nullptr, n, M, N, Kd,
@@ -2141,7 +2181,7 @@ bool Engine::Impl::gemv_group(const Tensor& a, const size_t* op_idx, int n, Tens
     static const bool w8_gemv = [] { const char* e = getenv("OSB_W8_GEMV"); return !(e && e[0] == '0'); }();
     static const bool grouped = [] { const char* e = getenv("OSB_GEMV_GROUPED"); return !(e && e[0] == '0'); }();
     if (!grouped) return false;
-    bool u8 = true, flt = true;
+    bool u8 = true, flt = true, f16w = true;
     for (int g = 0; g < n; g++) {
         const OpDef& op = E.m_ops[op_idx[g]];
         const TensorRef& wr = op.in[1];
@@ -2149,19 +2189,20 @@ bool Engine::Impl::gemv_group(const Tensor& a, const size_t* op_idx, int n, Tens
         const bool w_u8 = w8_gemv && wr.wtype == DType::u8 && rows <= 2 && wr.shape[1] % 16 == 0 && wr.shape[1] >= 256 && Kd >= 64 && weight_target(op, wr, false) == a.type;
         u8 = u8 && w_u8;
         flt = flt && (wr.wtype != DType::u8 || !w8_gemv) && wr.shape[1] % 8 == 0 && wr.shape[1] >= 256;
+        f16w = f16w && f16w_gemv(op, a);
     }
     if (!u8 && !flt) return false;
     const void* B[3]; void* C[3]; int64_t N[3]; float ws[3]; int wz[3];
     Tensor wt[3];
     for (int g = 0; g < n; g++) {
         const OpDef& op = E.m_ops[op_idx[g]];
-        wt[g] = u8 ? get_weight(op_idx[g], 1, false, false, true) : in(op_idx[g], 1);
-        if (!u8 && wt[g].type != a.type) wt[g] = convert(wt[g], a.type);
+        wt[g] = (u8 || f16w) ? get_weight(op_idx[g], 1, false, false, true) : in(op_idx[g], 1);
+        if (!u8 && !f16w && wt[g].type != a.type) wt[g] = convert(wt[g], a.type);
         std::vector<int64_t> os = a.shape; os.back() = op.in[1].shape[1];
         outs[g] = make(a.type, os);
         B[g] = wt[g].data(); C[g] = outs[g].mdata(); N[g] = op.in[1].shape[1]; ws[g] = wt[g].scale; wz[g] = wt[g].zero_point;
     }
-    const int rc = osb_gemv_grouped(a.data(), B, C, N, ws, wz, n, rows, Kd, u8 ? OSB_U8 : K(a.type), K(a.type), st);
+    const int rc = osb_gemv_grouped(a.data(), B, C, N, ws, wz, n, rows, Kd, u8 ? OSB_U8 : (f16w ? OSB_F16 : K(a.type)), K(a.type), st);
     if (rc == (int)cudaErrorNotSupported) return false;
     ck(rc, "osb_gemv_grouped");
     return true;

@@ -202,14 +202,17 @@ skinny_gemm_kernel(const T* __restrict__ A, const T* __restrict__ B, T* __restri
 // into (256-column x k-slice) panels so that ~2 waves of CTAs stream it with 16-byte loads; partial sums are reduced in
 // shared memory, then added with fp32 atomics into a zeroed scratch row; a second tiny kernel applies bias / residual and
 // rounds to the storage type.  Reads every weight exactly once.
+// The weight type W is the activation type T, or fp16 under fp32 activations: the weight stays as stored (8 columns per 16-byte load) and
+// is widened to fp32 in registers -- exactly the operand the reference gets when it converts an fp16 blob to fp32 at load time
+// (src/onnxstream.cpp:2892-2900) -- with fp32 FMA, sums, bias, residual and output: half the HBM bytes of the fp32 weight.
 constexpr int GEMV_U = 8;
 // CTAs a GEMV launch aims for (4 per SM); OSB_GEMV_CTAS overrides for tuning runs
 static inline int gemv_ctas() { static const int v = [] { const char* e = getenv("OSB_GEMV_CTAS"); int x = e ? atoi(e) : 0; return x > 0 ? x : 592; }(); return v; }
-template <typename T, int MAXM>
-__device__ __forceinline__ void gemv_panel_body(const T* __restrict__ A, const T* __restrict__ B, float* __restrict__ acc_out, int M, int N, int K, int k_per_cta,
+template <typename W, typename T, int MAXM>
+__device__ __forceinline__ void gemv_panel_body(const T* __restrict__ A, const W* __restrict__ B, float* __restrict__ acc_out, int M, int N, int K, int k_per_cta,
                                                 int* __restrict__ counter, T* __restrict__ C, const T* __restrict__ bias, const T* __restrict__ residual, int panel, int ldb)
 {
-    constexpr int VEC = 16 / sizeof(T);           // columns per thread
+    constexpr int VEC = 16 / sizeof(W);           // columns per thread
     constexpr int COLS = 32 * VEC;                // columns per CTA
     __shared__ float red[4][MAXM][COLS];
     const int cg = threadIdx.x & 31, kl = threadIdx.x >> 5;       // 32 column groups x 4 k-lanes
@@ -224,11 +227,11 @@ __device__ __forceinline__ void gemv_panel_body(const T* __restrict__ A, const T
         // GEMV_U independent 16-byte loads per thread before the first FMA: a decode GEMV is pure weight streaming and one load in
         // flight per thread leaves HBM bandwidth unused; 8 x 16 B x 128 threads x 4 CTAs = 64 KB in flight per SM
         for (int k = k_lo + kl; k < k_hi; k += 4 * GEMV_U) {
-            Vec<T, VEC> b[GEMV_U];
+            Vec<W, VEC> b[GEMV_U];
 #pragma unroll
             for (int u = 0; u < GEMV_U; u++) {
                 const int kk = k + 4 * u;
-                if (kk < k_hi) b[u] = load_vec<T, VEC>(B + (int64_t)kk * ldb + n0);
+                if (kk < k_hi) b[u] = load_vec<W, VEC>(B + (int64_t)kk * ldb + n0);
             }
 #pragma unroll
             for (int u = 0; u < GEMV_U; u++) {
@@ -283,13 +286,13 @@ __device__ __forceinline__ void gemv_panel_body(const T* __restrict__ A, const T
     if (threadIdx.x == 0) *counter = 0;
 }
 
-template <typename T, int MAXM>
+template <typename W, typename T, int MAXM>
 __global__ void __launch_bounds__(128)
-gemv_panel_kernel(const T* __restrict__ A, const T* __restrict__ B, float* __restrict__ acc_out, int M, int N, int K, int k_per_cta,
+gemv_panel_kernel(const T* __restrict__ A, const W* __restrict__ B, float* __restrict__ acc_out, int M, int N, int K, int k_per_cta,
                   int* __restrict__ counters, T* __restrict__ C, const T* __restrict__ bias, const T* __restrict__ residual, int ldb)
 {
     osb_pdl_prologue();
-    gemv_panel_body<T, MAXM>(A, B, acc_out, M, N, K, k_per_cta, counters + blockIdx.x, C, bias, residual, (int)blockIdx.x, ldb);
+    gemv_panel_body<W, T, MAXM>(A, B, acc_out, M, N, K, k_per_cta, counters + blockIdx.x, C, bias, residual, (int)blockIdx.x, ldb);
 }
 
 // Up to three GEMVs that share their input row(s) and K (q / k / v projections, gate / up of a gated MLP) as ONE launch: blockIdx.x walks
@@ -300,14 +303,14 @@ struct GemvGroups {
     float wscale[3]; int wzp[3];
     int groups;
 };
-template <typename T, int MAXM>
+template <typename W, typename T, int MAXM>
 __global__ void __launch_bounds__(128)
 gemv_panel_grouped_kernel(const T* __restrict__ A, GemvGroups g, float* __restrict__ acc_out, int M, int K, int k_per_cta, int* __restrict__ counters)
 {
     osb_pdl_prologue();
     const int bx = (int)blockIdx.x;
     const int gi = bx >= g.panel0[2] && g.groups > 2 ? 2 : (bx >= g.panel0[1] ? 1 : 0);
-    gemv_panel_body<T, MAXM>(A, (const T*)g.B[gi], acc_out + g.acc0[gi], M, g.N[gi], K, k_per_cta, counters + bx, (T*)g.C[gi], nullptr, nullptr, bx - g.panel0[gi], g.N[gi]);
+    gemv_panel_body<W, T, MAXM>(A, (const W*)g.B[gi], acc_out + g.acc0[gi], M, g.N[gi], K, k_per_cta, counters + bx, (T*)g.C[gi], nullptr, nullptr, bx - g.panel0[gi], g.N[gi]);
 }
 
 // The same panel GEMV with uint8 weights [K, N] (per-tensor scale / zero point), M <= 2: 16 columns per thread per 16-byte load, the
@@ -788,7 +791,7 @@ int osb_gemm_ld(const void* A, int64_t lda, const void* B, int64_t ldb, void* C,
         int k_per = (int)((K + gy - 1) / gy);
         gy = (int)((K + k_per - 1) / k_per);
         dim3 grid(gx, gy);
-#define OSB_GEMV(T_, MM_) osb_launch((gemv_panel_kernel<T_, MM_>), grid, 128, 0, st, (const T_*)A, (const T_*)B, scratch, (int)M, (int)N, (int)K, k_per, \
+#define OSB_GEMV(T_, MM_) osb_launch((gemv_panel_kernel<T_, T_, MM_>), grid, 128, 0, st, (const T_*)A, (const T_*)B, scratch, (int)M, (int)N, (int)K, k_per, \
                                     counters, (T_*)C, (const T_*)bias, (const T_*)residual, (int)ldb)
         // row-count instantiations: the M = 1 decode GEMV keeps 8 accumulators instead of 64
         if (dtype == OSB_F16) { if (M == 1) OSB_GEMV(__half, 1); else if (M == 2) OSB_GEMV(__half, 2); else if (M <= 4) OSB_GEMV(__half, 4); else OSB_GEMV(__half, 8); }
@@ -827,17 +830,38 @@ int osb_gemv_w8(const void* A, const void* Wq, void* C, const void* bias, const 
     return launched();
 }
 
+// y[M,N] = x[M,K] . W[K,N] (+ bias, + residual), M <= 8, fp32 activations / bias / residual / output, fp16 weights (row stride ldb)
+// widened in registers (see gemv_panel_body).  cudaErrorNotSupported = shape outside the panel kernel (the caller converts the weight).
+int osb_gemv_f16w(const void* A, const void* W, int64_t ldb, void* C, const void* bias, const void* residual, int64_t M, int64_t N, int64_t K, void* stream)
+{
+    if (M < 1 || M > 8 || N < 256 || K < 64 || ldb < N || ldb % 8 || !aligned16(W)) return (int)cudaErrorNotSupported;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int cols = 256;
+    const int gx = (int)((N + cols - 1) / cols);
+    OsbWorkspace* ws = (gx <= 4096 && (size_t)M * N <= OSB_WS_GEMV_FLOATS) ? osb_workspace(st, OSB_WS_GEMV) : nullptr;
+    if (!ws) return (int)cudaErrorNotSupported;
+    int gy = (int)max<int64_t>(1, min<int64_t>((K + 15) / 16, (gemv_ctas() + gx - 1) / gx));
+    int k_per = (int)((K + gy - 1) / gy);
+    gy = (int)((K + k_per - 1) / k_per);
+    dim3 grid(gx, gy);
+#define OSB_GEMVH(MM_) osb_launch((gemv_panel_kernel<__half, float, MM_>), grid, 128, 0, st, (const float*)A, (const __half*)W, ws->gemv, (int)M, (int)N, (int)K, k_per, \
+                                  ws->gemv_counters, (float*)C, (const float*)bias, (const float*)residual, (int)ldb)
+    if (M == 1) OSB_GEMVH(1); else if (M == 2) OSB_GEMVH(2); else if (M <= 4) OSB_GEMVH(4); else OSB_GEMVH(8);
+#undef OSB_GEMVH
+    return launched();
+}
+
 // groups (2 or 3) GEMVs y_g[M,N_g] = x[M,K] . W_g[K,N_g] sharing x, as one launch.  wdtype == OSB_U8: uint8 weights dequantised in
-// registers (M <= 2); otherwise weights of the activation type.  cudaErrorNotSupported = shape outside what the grouped kernels cover
+// registers (M <= 2); wdtype == OSB_F16 with dtype == OSB_F32: fp16 weights widened in registers; otherwise weights of the activation type.  cudaErrorNotSupported = shape outside what the grouped kernels cover
 // (the caller launches the GEMVs one by one).
 int osb_gemv_grouped(const void* A, const void* const* B, void* const* C, const int64_t* N, const float* wscale, const int* wzp, int groups,
                      int64_t M, int64_t K, int wdtype, int dtype, void* stream)
 {
     if (groups < 2 || groups > 3 || (dtype != OSB_F16 && dtype != OSB_F32) || M < 1 || K < 64) return (int)cudaErrorNotSupported;
     const bool w8 = wdtype == OSB_U8;
-    if (!w8 && wdtype != dtype) return (int)cudaErrorNotSupported;
+    if (!w8 && wdtype != dtype && !(wdtype == OSB_F16 && dtype == OSB_F32)) return (int)cudaErrorNotSupported;
     if (M > (w8 ? 2 : 8)) return (int)cudaErrorNotSupported;
-    const int cols = w8 ? 512 : (dtype == OSB_F16 ? 256 : 128);
+    const int cols = w8 ? 512 : (wdtype == OSB_F16 ? 256 : 128);
     GemvGroups g{};
     g.groups = groups;
     int panels = 0; int64_t acc = 0;
@@ -861,9 +885,10 @@ int osb_gemv_grouped(const void* A, const void* const* B, void* const* C, const 
         if (dtype == OSB_F16) osb_launch((gemv_w8_panel_grouped_kernel<__half>), grid, 128, 0, st, (const __half*)A, g, ws->gemv, (int)M, (int)K, k_per, ws->gemv_counters);
         else osb_launch((gemv_w8_panel_grouped_kernel<float>), grid, 128, 0, st, (const float*)A, g, ws->gemv, (int)M, (int)K, k_per, ws->gemv_counters);
     } else {
-#define OSB_GEMVG(T_, MM_) osb_launch((gemv_panel_grouped_kernel<T_, MM_>), grid, 128, 0, st, (const T_*)A, g, ws->gemv, (int)M, (int)K, k_per, ws->gemv_counters)
-        if (dtype == OSB_F16) { if (M == 1) OSB_GEMVG(__half, 1); else if (M == 2) OSB_GEMVG(__half, 2); else if (M <= 4) OSB_GEMVG(__half, 4); else OSB_GEMVG(__half, 8); }
-        else { if (M == 1) OSB_GEMVG(float, 1); else if (M == 2) OSB_GEMVG(float, 2); else if (M <= 4) OSB_GEMVG(float, 4); else OSB_GEMVG(float, 8); }
+#define OSB_GEMVG(W_, T_, MM_) osb_launch((gemv_panel_grouped_kernel<W_, T_, MM_>), grid, 128, 0, st, (const T_*)A, g, ws->gemv, (int)M, (int)K, k_per, ws->gemv_counters)
+        if (dtype == OSB_F16) { if (M == 1) OSB_GEMVG(__half, __half, 1); else if (M == 2) OSB_GEMVG(__half, __half, 2); else if (M <= 4) OSB_GEMVG(__half, __half, 4); else OSB_GEMVG(__half, __half, 8); }
+        else if (wdtype == OSB_F16) { if (M == 1) OSB_GEMVG(__half, float, 1); else if (M == 2) OSB_GEMVG(__half, float, 2); else if (M <= 4) OSB_GEMVG(__half, float, 4); else OSB_GEMVG(__half, float, 8); }
+        else { if (M == 1) OSB_GEMVG(float, float, 1); else if (M == 2) OSB_GEMVG(float, float, 2); else if (M <= 4) OSB_GEMVG(float, float, 4); else OSB_GEMVG(float, float, 8); }
 #undef OSB_GEMVG
     }
     return launched();
