@@ -53,6 +53,14 @@ int osb_tc_conv_f32x_ok(int64_t H, int64_t W, int64_t Cin, int64_t Cout, int kh,
 int osb_tc_gemm_f32x(const void* A6, const void* B6, void* C_f32, const void* bias_f32, const void* residual_f32, int64_t M, int64_t N, int64_t K6, int b_transposed, void* stream);
 int osb_tc_conv_f32x(const void* x6, const void* w6, const void* bias_f32, const void* residual_f32, void* y_f32, int64_t H, int64_t W, int64_t Cin6, int64_t Cout,
                      int kh, int kw, int stride, int pad_top, int pad_left, int64_t Ho, int64_t Wo, void* stream);
+/* fp32 MatMul on an fp16 weight read as stored: C [M, N] = A [M, K] . float(B) + bias [N] + residual [M, N], A / C / bias / residual fp32, B fp16
+   [K, N] with rows ldb elements apart.  The fp16 weight is exactly hi + lo in bf16, split in shared memory, so the five nonzero products of the
+   triple split above run with no expanded weight (5/6 of the tensor-core work).  planes: scratch of 6 M K bytes, 16-byte aligned, for the
+   bf16 planes of A.  cudaErrorNotSupported (801), nothing launched: K % 8, ldb % 8, ldb < N, unaligned A / B / planes (16 bytes) or C /
+   bias / residual (4 bytes), no workspace. */
+int osb_tc_gemm_f32x_f16w_ok(int64_t M, int64_t N, int64_t K, int64_t ldb);
+int osb_tc_gemm_f32x_f16w(const void* A_f32, const void* B_f16, int64_t ldb, void* C_f32, const void* bias_f32, const void* residual_f32, int64_t M, int64_t N,
+                          int64_t K, void* planes, void* stream);
 /* Concat of two tensors along one axis in one launch (src/onnxstream.cpp Concat branch, two inputs): outer slices of a_bytes / b_bytes each.
    cudaErrorNotSupported (801) unless both slice sizes and all three pointers are multiples of 16 bytes. */
 int osb_concat2(const void* a, const void* b, void* out, int64_t outer, int64_t a_bytes, int64_t b_bytes, void* stream);

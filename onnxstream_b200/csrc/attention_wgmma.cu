@@ -1489,6 +1489,13 @@ int sdpa_f32x_launch(const float* q, const float* k, const float* v, SdpaF32xPar
 
 }  // namespace
 
+// fp32 rows [rows][C] -> bf16 planes [rows][3][C] (h, m, l), C % 4 == 0, 16-byte aligned: the A operand of osb_tc_gemm_f32x_f16w
+int osb_f32x_split_rows(const float* x, __nv_bfloat16* planes, int64_t rows, int64_t C, cudaStream_t st)
+{
+    osb_launch((f32x_split_kernel), grid_for((size_t)(rows * C / 4), 256), 256, 0, st, x, C, x, C, x, C, planes, planes, planes, rows, (int64_t)0, (int)C);
+    return launched();
+}
+
 extern "C" int osb_flash_attention_ok(int64_t T, int64_t Tk, int64_t d, int dtype)
 {
     return dtype == OSB_F16 && T >= 64 && fa_dims_ok(T, Tk, d) && get_encode() != nullptr;

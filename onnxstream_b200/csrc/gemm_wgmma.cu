@@ -500,6 +500,180 @@ __global__ void splitk_reduce_f32_kernel(const float* __restrict__ ws, float* __
     }
 }
 
+
+// ---- fp32 activations x an fp16 weight read in place (osb_tc_gemm_f32x_f16w) --------------------------------------------------------
+// An fp16 value w is exactly hi + lo with hi = bf16(w) and lo = bf16(w - hi) (the remainder has at most 3 significant bits, and fp16
+// subnormals are bf16 normals), so the bf16 triple split of the widened weight is (hi, lo, 0): of the six products of the fp32 path (hh,
+// hm, mh, hl, lh, mm; osb_tc_gemm_f32x) hl is zero, and five remain.  One 128 x 128 tile per CTA, 384 threads, persistent:
+//   warp 0            TMA producer: per raw k-block (64 of K) the three bf16 planes of A ([M][3][K], one map over [M, 3 K]: plane p's
+//                     k-block kc at column p K + kc; a chunk past K reads the next plane against B rows that TMA zero-fills) and the fp16
+//                     B block as stored (two 64-column atoms, MN-major), which completes `landed`
+//   warps 1-3         B splitters: every fp16 element of the block once -> hi in place and lo into the stage's second B buffer (elementwise
+//                     at the same offset, so the 128B swizzle carries over), fence.proxy.async, arrive on `full` (one per warp)
+//   warpgroups 1, 2   consumers: per stage the five products (h, hi), (h, lo), (m, hi), (l, hi), (m, lo) as 5 x 4 wgmma m64n128k16 into
+//                     the fp32 accumulators, one stage in flight; the tile's raw fp32 sums go to the split-K workspace [split][M][N] and
+//                     splitk_reduce_f32_kernel adds the splits, fp32 bias and residual.
+// Each raw B block is converted once and its 16 KB read from L2 once; a stage is 48 KB of A planes + 32 KB of B parts, 2 stages.
+namespace f16w {
+constexpr int A_PLANE_BYTES = BLOCK_M * BLOCK_K * 2;            // 16 KB
+constexpr int A_BYTES = 3 * A_PLANE_BYTES;
+constexpr int B_PART_BYTES = BLOCK_N * BLOCK_K * 2;             // 16 KB
+constexpr int B_BYTES = 2 * B_PART_BYTES;
+constexpr int STAGES = 2;
+constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int SPLIT_THREADS = 96;
+}
+
+// two fp16 values (one 32-bit word) -> their bf16 hi and lo parts
+__device__ __forceinline__ void f16x2_bf16_parts(uint32_t v, uint32_t& hi, uint32_t& lo)
+{
+    const float2 x = __half22float2(*reinterpret_cast<const __half2*>(&v));
+    const __nv_bfloat162 h = __float22bfloat162_rn(x);
+    const float2 hf = __bfloat1622float2(h);
+    const __nv_bfloat162 l = __float22bfloat162_rn(make_float2(x.x - hf.x, x.y - hf.y));
+    hi = *reinterpret_cast<const uint32_t*>(&h);
+    lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+// p: M, N, K, m_tiles, n_tiles, k_blocks_per_tap (= ceil(K / 64)), split_k, ws
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const TcParams p)
+{
+    using namespace f16w;
+    osb_pdl_trigger_entry();
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem_a = smem;                             // [STAGES][3 planes][128 rows][64]
+    uint8_t* smem_b = smem + STAGES * A_BYTES;          // [STAGES][hi, lo][2 atoms][64 k][64]
+    uint64_t* bars = (uint64_t*)(smem + STAGES * (A_BYTES + B_BYTES));
+    uint64_t* full = bars;
+    uint64_t* empty = bars + STAGES;
+    uint64_t* landed = bars + 2 * STAGES;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp == 0 && lane == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
+    }
+    if (warp == 1 && lane == 0) {
+        for (int i = 0; i < STAGES; i++) { mbar_init(&full[i], 3); mbar_init(&empty[i], CONSUMER_THREADS); mbar_init(&landed[i], 1); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    osb_pdl_wait();     // the planes of A are written by the split launched just before
+
+    const int tiles = p.m_tiles * p.n_tiles;
+    const int total = tiles * p.split_k;
+    const int kbk = p.k_blocks_per_tap;
+    const int kb_per_split = (kbk + p.split_k - 1) / p.split_k;   // host guarantees every split runs >= 1 k-block
+
+    if (warp == 0) {
+        // ===================== TMA producer =====================
+        const uint32_t sa0 = smem_u32(smem_a), sb0 = smem_u32(smem_b);
+        int stage = 0; uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+            const int sp = tile % p.split_k, r = tile / p.split_k;
+            const int m0 = (r % p.m_tiles) * BLOCK_M, n0 = (r / p.m_tiles) * BLOCK_N;
+            const int kb_lo = sp * kb_per_split, kb_hi = min(kb_lo + kb_per_split, kbk);
+            for (int kb = kb_lo; kb < kb_hi; kb++) {
+                mbar_wait(&empty[stage], phase ^ 1);
+                if (elect_one()) {
+                    mbar_expect_tx(&landed[stage], A_BYTES + B_PART_BYTES);
+                    const int kc = kb * BLOCK_K;
+                    const uint32_t sa = sa0 + stage * A_BYTES, sb = sb0 + stage * B_BYTES;
+#pragma unroll
+                    for (int pl = 0; pl < 3; pl++) tma_load_3d_s(sa + pl * A_PLANE_BYTES, &map_a, &landed[stage], pl * p.K + kc, m0, 0);
+#pragma unroll
+                    for (int at = 0; at < 2; at++) tma_load_3d_s(sb + at * 8192, &map_b, &landed[stage], n0 + 64 * at, kc, 0);
+                }
+                __syncwarp();
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+        }
+        osb_pdl_trigger_late();
+    } else if (warp < 4) {
+        // ===================== B splitters: fp16 -> hi (in place) and lo, once per raw block =====================
+        const int t = (int)threadIdx.x - 32;
+        constexpr int PER = (B_PART_BYTES / 16 + SPLIT_THREADS - 1) / SPLIT_THREADS;
+        int stage = 0; uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+            const int sp = tile % p.split_k;
+            const int kb_lo = sp * kb_per_split, kb_hi = min(kb_lo + kb_per_split, kbk);
+            for (int kb = kb_lo; kb < kb_hi; kb++) {
+                mbar_wait(&landed[stage], phase);
+                uint4* bh = reinterpret_cast<uint4*>(smem_b + stage * B_BYTES);
+                uint4* bl = reinterpret_cast<uint4*>(smem_b + stage * B_BYTES + B_PART_BYTES);
+                uint4 v[PER];
+#pragma unroll
+                for (int j = 0; j < PER; j++) if (t + j * SPLIT_THREADS < B_PART_BYTES / 16) v[j] = bh[t + j * SPLIT_THREADS];
+#pragma unroll
+                for (int j = 0; j < PER; j++) {
+                    const int i = t + j * SPLIT_THREADS;
+                    if (i >= B_PART_BYTES / 16) continue;
+                    uint4 h, l;
+                    f16x2_bf16_parts(v[j].x, h.x, l.x); f16x2_bf16_parts(v[j].y, h.y, l.y);
+                    f16x2_bf16_parts(v[j].z, h.z, l.z); f16x2_bf16_parts(v[j].w, h.w, l.w);
+                    bh[i] = h; bl[i] = l;
+                }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor cores
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&full[stage]);
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+        }
+    } else {
+        // ===================== consumers: 5 products per stage, fp32 partials out =====================
+        const int wg = (warp >> 2) - 1;
+        const uint64_t adesc0 = make_smem_desc(smem_u32(smem_a) + 64 * wg * 128, 16, 1024);
+        const uint64_t bdesc0 = make_smem_desc(smem_u32(smem_b), 8192, 1024);
+        constexpr uint64_t AP = A_PLANE_BYTES >> 4, BP = B_PART_BYTES >> 4;   // descriptor units (16 B)
+        const int r_lo = 64 * wg + (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
+        const bool pair_ok = (p.N & 1) == 0;
+        int stage = 0; uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+            const int sp = tile % p.split_k, r = tile / p.split_k;
+            const int m0 = (r % p.m_tiles) * BLOCK_M, n0 = (r / p.m_tiles) * BLOCK_N;
+            const int kb_lo = sp * kb_per_split, kb_hi = min(kb_lo + kb_per_split, kbk);
+            float acc[64];
+#pragma unroll
+            for (int i = 0; i < 64; i++) acc[i] = 0.f;
+            int prev = -1;
+            for (int kb = kb_lo; kb < kb_hi; kb++) {
+                mbar_wait(&full[stage], phase);
+                const uint64_t a = adesc0 + (uint64_t)(stage * (A_BYTES >> 4)), b = bdesc0 + (uint64_t)(stage * (B_BYTES >> 4));
+                // (A plane, B part): (h, hi), (h, lo), (m, hi), (l, hi), (m, lo)
+                const uint64_t ad[5] = { a, a, a + AP, a + 2 * AP, a + AP }, bd[5] = { b, b + BP, b, b, b + BP };
+                wgmma_fence();
+#pragma unroll
+                for (int x = 0; x < 5; x++) {
+#pragma unroll
+                    for (int k = 0; k < BLOCK_K / WG_K; k++)
+                        wgmma_ss<128, 1, true>(acc, ad[x] + (uint64_t)(k * ((WG_K * 2) >> 4)), bd[x] + (uint64_t)(k * ((WG_K * 128) >> 4)), 1u);
+                }
+                wgmma_commit();
+                if (prev >= 0) { wgmma_wait<1>(); mbar_arrive(&empty[prev]); }
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            mbar_arrive(&empty[prev]);
+            // raw fp32 sums of this split -> ws[sp][M][N]
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int m = m0 + r_lo + 8 * h;
+                if (m >= p.M) continue;
+                float* wrow = p.ws + ((long long)sp * p.M + m) * p.N;
+#pragma unroll
+                for (int j = 0; j < 16; j++) {
+                    const int n = n0 + 8 * j + cq;
+                    const float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                    if (n + 1 < p.N && pair_ok) *reinterpret_cast<float2*>(wrow + n) = make_float2(f0, f1);
+                    else { if (n < p.N) wrow[n] = f0; if (n + 1 < p.N) wrow[n + 1] = f1; }
+                }
+            }
+        }
+    }
+}
+
 #include "gemm_i8.cuh"
 
 // ---- host side -------------------------------------------------------------------------------------------------
@@ -1143,15 +1317,18 @@ int osb_tc_conv_launch(const void* x, const void* w, const void* bias, const voi
 // A to [h|h|m|h|l|m] and B to [h|m|h|l|h|m] along K (osb_bf16x3_expand_*), products are exact in fp32 and accumulate in the fp32 register
 // accumulator.  A, B: bf16 expansions (K6 = 6 K); C, bias, residual: fp32; C dense [M][N].  cudaErrorNotSupported: run the CUDA-core kernel.
 // shape predicates of the fp32 tensor-core path (before the caller spends time expanding operands)
-extern "C" int osb_tc_gemm_f32x_ok(int64_t M, int64_t N, int64_t K)
+static bool f32_tc_on()
 {
     static const bool on = [] { const char* e = getenv("OSB_F32_TC"); return !(e && e[0] == '0'); }();
-    return on && M >= 32 && N >= 8 && N % 8 == 0 && K >= 8 && (6 * K) % 8 == 0 && (size_t)M * N * 4 <= WS_MAX && get_encode() != nullptr ? 1 : 0;
+    return on;
+}
+extern "C" int osb_tc_gemm_f32x_ok(int64_t M, int64_t N, int64_t K)
+{
+    return f32_tc_on() && M >= 32 && N >= 8 && N % 8 == 0 && K >= 8 && (6 * K) % 8 == 0 && (size_t)M * N * 4 <= WS_MAX && get_encode() != nullptr ? 1 : 0;
 }
 extern "C" int osb_tc_conv_f32x_ok(int64_t H, int64_t W, int64_t Cin, int64_t Cout, int kh, int kw, int stride, int64_t Ho, int64_t Wo)
 {
-    static const bool on = [] { const char* e = getenv("OSB_F32_TC"); return !(e && e[0] == '0'); }();
-    return on && (6 * Cin) % 8 == 0 && 6 * Cin >= 16 && stride >= 1 && stride <= 2 && H * W >= 64 && kh <= 7 && kw <= 7 && (size_t)Ho * Wo * Cout * 4 <= WS_MAX &&
+    return f32_tc_on() && (6 * Cin) % 8 == 0 && 6 * Cin >= 16 && stride >= 1 && stride <= 2 && H * W >= 64 && kh <= 7 && kw <= 7 && (size_t)Ho * Wo * Cout * 4 <= WS_MAX &&
            get_encode() != nullptr ? 1 : 0;
 }
 
@@ -1174,4 +1351,61 @@ extern "C" int osb_tc_conv_f32x(const void* x6, const void* w6, const void* bias
     int r = osb_tc_conv_launch(x6, w6, bias, residual, y, H, W, Cin6, Cout, kh, kw, stride, pad_top, pad_left, Ho, Wo, (cudaStream_t)stream, nullptr, nullptr, 0, nullptr);
     g_f32x = 0;
     return r;
+}
+
+// ---- fp32 GEMM on an fp16 weight read in place ------------------------------------------------------------------------------------------
+int osb_f32x_split_rows(const float* x, __nv_bfloat16* planes, int64_t rows, int64_t C, cudaStream_t st);   // attention_wgmma.cu
+
+extern "C" int osb_tc_gemm_f32x_f16w_ok(int64_t M, int64_t N, int64_t K, int64_t ldb)
+{
+    return f32_tc_on() && M >= 1 && N >= 1 && K >= 8 && K % 8 == 0 && ldb % 8 == 0 && ldb >= N && M <= (1 << 30) && ldb <= (1 << 30) &&
+           3 * K <= (1 << 30) && (size_t)N * 4 * BLOCK_M <= WS_MAX && get_encode() != nullptr ? 1 : 0;
+}
+
+// C [M, N] fp32 = A [M, K] fp32 . B [K, N] fp16 (rows ldb apart) + bias [N] + residual [M, N] (fp32, either may be null): the split of A into
+// `planes`, then tc_gemm_f16w_kernel and the fp32 reduce, once per block of rows whose fp32 partials fit the workspace.
+extern "C" int osb_tc_gemm_f32x_f16w(const void* A, const void* B, int64_t ldb, void* C, const void* bias, const void* residual, int64_t M, int64_t N,
+                                     int64_t K, void* planes, void* stream)
+{
+    if (!osb_tc_gemm_f32x_f16w_ok(M, N, K, ldb) || !aligned16(A) || !aligned16(B) || !aligned16(planes) || ((uintptr_t)C & 3) || ((uintptr_t)bias & 3) ||
+        ((uintptr_t)residual & 3))
+        return (int)cudaErrorNotSupported;
+    cudaStream_t st = (cudaStream_t)stream;
+    OsbWorkspace* wsp = osb_workspace(st, OSB_WS_SPLITK);
+    if (!wsp) return (int)cudaErrorNotSupported;
+    const int64_t rows_max = std::min<int64_t>(M, (int64_t)(WS_MAX / ((size_t)N * 4)) / BLOCK_M * BLOCK_M);
+    const int64_t K3 = 3 * K, kbk = (K + BLOCK_K - 1) / BLOCK_K;
+    const __nv_bfloat16* pl = (const __nv_bfloat16*)planes;
+    CUtensorMap mb;
+    int sw = 0;
+    if (!make_map_rb(&mb, B, (uint64_t)N, (uint64_t)K, 1, (uint64_t)ldb * 2, (uint64_t)(K * ldb) * 2, 64, BLOCK_K, &sw)) return (int)cudaErrorNotSupported;
+    std::vector<CUtensorMap> ma((size_t)((M + rows_max - 1) / rows_max));
+    for (size_t i = 0; i < ma.size(); i++) {
+        const int64_t m0 = (int64_t)i * rows_max, rows = std::min(rows_max, M - m0);
+        if (!make_map_rb(&ma[i], pl + m0 * K3, (uint64_t)K3, (uint64_t)rows, 1, (uint64_t)K3 * 2, (uint64_t)(rows * K3) * 2, BLOCK_K, BLOCK_M, &sw))
+            return (int)cudaErrorNotSupported;
+    }
+    static const cudaError_t attr = cudaFuncSetAttribute(tc_gemm_f16w_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, f16w::SMEM_BYTES);
+    if (attr != cudaSuccess) return (int)attr;
+    int e = osb_f32x_split_rows((const float*)A, (__nv_bfloat16*)planes, M, K, st);
+    if (e) return e;
+    for (size_t i = 0; i < ma.size(); i++) {
+        const int64_t m0 = (int64_t)i * rows_max, rows = std::min(rows_max, M - m0);
+        TcParams p{};
+        p.M = (int)rows; p.N = (int)N; p.K = (int)K; p.batch = 1;
+        p.m_tiles = (int)((rows + BLOCK_M - 1) / BLOCK_M); p.n_tiles = (int)((N + BLOCK_N - 1) / BLOCK_N);
+        p.k_blocks_per_tap = (int)kbk;
+        // the fp32 path's split rule (old_split) over the raw k-blocks, each five products deep
+        p.split_k = choose_tile(TileProblem{ (int)rows, (int)N, 0, 0, 0, 1, (int)kbk, 0, true, true }).split;
+        if ((size_t)p.split_k * rows * N * 4 > WS_MAX) p.split_k = 1;
+        p.ws = wsp->splitk;
+        const int grid = (int)std::min<int64_t>((int64_t)p.m_tiles * p.n_tiles * p.split_k, num_sms());
+        osb_launch((tc_gemm_f16w_kernel), grid, NUM_THREADS, (size_t)f16w::SMEM_BYTES, st, ma[i], mb, p);
+        if ((e = launched(1))) return e;
+        const long long total = rows * N;
+        osb_launch((splitk_reduce_f32_kernel), (int)std::min<long long>((total + 255) / 256, num_sms() * 8), 256, 0, st, (const float*)p.ws,
+                   (float*)C + m0 * N, (const float*)bias, residual ? (const float*)residual + m0 * N : nullptr, (long long)rows, (int)N, p.split_k);
+        if ((e = launched())) return e;
+    }
+    return 0;
 }
