@@ -700,8 +700,10 @@ __global__ void attention_rows_kernel(const T* __restrict__ q, const T* __restri
                 logit = dot;
             }
             float mnew = fmaxf(m, warp_max(logit));
-            float corr = expf(m - mnew);
-            float p = s < Tk ? expf(logit - mnew) : 0.f;
+            // mnew = -inf only while every key so far is masked with -inf: keep acc and l at 0 (expf(-inf + inf) would be NaN)
+            const bool none = mnew == -INFINITY;
+            float corr = none ? 1.f : expf(m - mnew);
+            float p = (s < Tk && !none) ? expf(logit - mnew) : 0.f;
             l = l * corr + warp_sum(p);
             // acc = acc * corr + sum_s p_s * v[s]   (p staged through shared memory: trip counts differ per lane)
             ps[lane] = p;

@@ -114,7 +114,8 @@ def _check(o, q, k, v, h, d):
 # 64^2, 20 at 32^2), and ragged T / Tk that end inside a query tile and a key tile at every tile configuration
 SHAPES = [(4096, 4096, 8, 40), (4096, 77, 8, 40), (1024, 1024, 8, 80), (1024, 77, 8, 80), (256, 256, 8, 160), (256, 77, 8, 160),
           (64, 64, 8, 160), (64, 77, 8, 160), (4096, 77, 10, 64), (1024, 1024, 20, 64), (200, 77, 4, 80), (300, 200, 3, 128),
-          (130, 333, 2, 160), (96, 100, 2, 72), (65, 30, 2, 136), (320, 1000, 2, 48), (1, 5, 1, 8), (77, 77, 2, 16), (129, 65, 3, 56)]
+          (130, 333, 2, 160), (96, 100, 2, 72), (65, 30, 2, 136), (320, 1000, 2, 48), (1, 5, 1, 8), (77, 77, 2, 16), (129, 65, 3, 56)] + \
+    [(100, 77, 2, d) for d in range(8, 161, 8)]     # every accepted head dim on one ragged shape
 
 
 @pytest.mark.parametrize("T,Tk,h,d", SHAPES)

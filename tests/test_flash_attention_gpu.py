@@ -1,5 +1,5 @@
 """The fused multi-head flash attention (osb_flash_attention) at every head dim the SD 1.5 UNet uses (40, 80, 160) and at d = 128:
-the kernel against fp64 math at the UNet's shapes and at ragged ones, the scope osb_flash_attention_ok accepts, bit-identical repeat
+the kernel against fp64 math at the UNet's shapes, at ragged ones, at every accepted head dim and on rows of very different scale, the scope osb_flash_attention_ok accepts, bit-identical repeat
 launches, and a small UNet whose attention levels have d = 80 and d = 160 -- that it takes the flash route and matches the reference
 (stored reference output under tests/golden/oracle, tests/util.py)."""
 import ctypes
@@ -34,14 +34,19 @@ def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def _inputs(T, Tk, h, d):
+def _inputs(T, Tk, h, d, row_scales=False):
+    """q [T, h*d], k / v [Tk, h*d] fp16.  row_scales: query rows spread over three decades (|q| stays below 1e3, well inside fp16) and
+    key rows whose norm grows along the sequence, so the rows' maxima keep moving to later key tiles."""
     import torch
     C = h * d
     g = torch.Generator(device="cuda").manual_seed(T * 5 + Tk * 3 + d)
-    q = torch.randn(T, C, device="cuda", generator=g).half()
-    k = torch.randn(Tk, C, device="cuda", generator=g).half()
-    v = torch.randn(Tk, C, device="cuda", generator=g).half()
-    return q, k, v
+    q = torch.randn(T, C, device="cuda", generator=g)
+    k = torch.randn(Tk, C, device="cuda", generator=g)
+    v = torch.randn(Tk, C, device="cuda", generator=g)
+    if row_scales:
+        q *= torch.logspace(-1, 2, T, device="cuda")[torch.randperm(T, device="cuda", generator=g)].view(T, 1)
+        k *= torch.linspace(0.25, 2.0, Tk, device="cuda").view(Tk, 1)
+    return q.half(), k.half(), v.half()
 
 
 def _flash(K, q, k, v, T, Tk, h, d):
@@ -54,20 +59,19 @@ def _flash(K, q, k, v, T, Tk, h, d):
     return o
 
 
-# SD 1.5 UNet levels (8 heads: 64^2 d 40, 32^2 d 80, 16^2 and 8^2 d 160; self-attention and the 77-token context), d = 128, and ragged
-# T / Tk that end inside a query tile and a key tile
+# SD 1.5 UNet levels (8 heads: 64^2 d 40, 32^2 d 80, 16^2 and 8^2 d 160; self-attention and the 77-token context), d = 128, ragged
+# T / Tk that end inside a query tile and a key tile, and every head dim the kernel accepts (8 to 160: instantiations change at 48 / 64 /
+# 80 / 128)
 SHAPES = [(4096, 77, 8, 40), (1024, 1024, 8, 80), (1024, 77, 8, 80), (256, 256, 8, 160), (256, 77, 8, 160), (64, 64, 8, 160),
           (64, 77, 8, 160), (512, 512, 4, 128), (200, 77, 4, 80), (300, 200, 3, 128), (130, 333, 2, 160), (96, 100, 2, 72),
-          (64, 30, 2, 136), (320, 1000, 2, 48)]
+          (64, 30, 2, 136), (320, 1000, 2, 48)] + [(100, 77, 2, d) for d in range(8, 161, 8)]     # every accepted head dim, one ragged shape
 
 
-@pytest.mark.parametrize("T,Tk,h,d", SHAPES)
-def test_flash_attention_head_dims(K, T, Tk, h, d):
+def _check(o, q, k, v, h, d):
     """Against softmax(QK^T s)V in fp64 on the fp16-rounded operands, with the bar of test_kernels_gpu.py::test_flash_attention: P is
     rounded to fp16 before the second MMA, so |err| <= 2^-8 * sum|p_i v_i| + 2^-9 |ref| + 1e-4."""
     import torch
-    q, k, v = _inputs(T, Tk, h, d)
-    o = _flash(K, q, k, v, T, Tk, h, d)
+    T, Tk = q.shape[0], k.shape[0]
     qh = q.double().view(T, h, d).permute(1, 0, 2); kh = k.double().view(Tk, h, d).permute(1, 0, 2); vh = v.double().view(Tk, h, d).permute(1, 0, 2)
     P = torch.softmax(qh @ kh.transpose(1, 2) / d ** 0.5, dim=-1)
     ref = (P @ vh).permute(1, 0, 2).reshape(T, h * d)
@@ -76,6 +80,19 @@ def test_flash_attention_head_dims(K, T, Tk, h, d):
     tol = absref * 2.0 ** -8 + ref.abs() * 2.0 ** -9 + 1e-4
     assert not torch.isnan(o).any()
     assert not (err > tol).any(), f"max err {float(err.max()):.4g}, ref max {float(ref.abs().max()):.4g}, bad {(err > tol).sum().item()}"
+
+
+@pytest.mark.parametrize("T,Tk,h,d", SHAPES)
+def test_flash_attention_head_dims(K, T, Tk, h, d):
+    q, k, v = _inputs(T, Tk, h, d)
+    _check(_flash(K, q, k, v, T, Tk, h, d), q, k, v, h, d)
+
+
+@pytest.mark.parametrize("T,Tk,h,d", [(1000, 1000, 2, 40), (333, 777, 2, 80), (500, 500, 2, 128), (256, 1024, 1, 160)])
+def test_flash_attention_running_max(K, T, Tk, h, d):
+    """Rows of very different scale: a kernel that kept the first tile's maximum or skipped the rescaling of O fails."""
+    q, k, v = _inputs(T, Tk, h, d, row_scales=True)
+    _check(_flash(K, q, k, v, T, Tk, h, d), q, k, v, h, d)
 
 
 def test_flash_attention_scope(K):

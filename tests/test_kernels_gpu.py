@@ -694,12 +694,21 @@ ATTN_CASES = [
     (4, 3, 515, 80, 40, 1, True, F16),        # several query rows, d != dv, not a multiple of 8 halves per lane chunk
     (6, 2, 257, 20, 20, 3, True, F32),
     (4, 1, 100, 64, 64, 2, True, F16),        # short key axis: one warp per row
+    # -inf masks (test_node_kernels_gpu.neg_inf_mask): whole 32-key warps and whole 128-key splits with no finite key
+    (32, 1, 2048, 64, 64, 8, "ninf_lead40", F16),
+    (32, 1, 2048, 64, 64, 8, "ninf_splits", F32),
+    (32, 1, 2048, 64, 64, 8, "ninf_splits", F16),
+    (4, 3, 515, 80, 40, 1, "ninf_splits", F32),
+    (8, 1, 300, 64, 64, 2, "ninf_one_key", F16),
+    (6, 2, 257, 20, 20, 3, "ninf_one_key", F32),
+    (4, 1, 100, 64, 64, 2, "ninf_lead40", F32),   # short key axis: the per-row kernel
 ]
 
 
 @pytest.mark.parametrize("heads,Tq,Tk,d,dv,group,with_mask,dtype", ATTN_CASES)
 def test_attention_decode_matches_fp64(K, heads, Tq, Tk, d, dv, group, with_mask, dtype):
     import torch
+    from test_node_kernels_gpu import NEG_INF_MASKS, neg_inf_mask
     K.osb_attention.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_int64] * 5 + [ctypes.c_float, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_void_p]
     ty = torch.float16 if dtype == F16 else torch.float32
     g = torch.Generator(device="cuda").manual_seed(heads * 1000 + Tk)
@@ -707,7 +716,9 @@ def test_attention_decode_matches_fp64(K, heads, Tq, Tk, d, dv, group, with_mask
     k = torch.randn(heads // group, Tk, d, device="cuda", generator=g).to(ty)
     v = torch.randn(heads // group, Tk, dv, device="cuda", generator=g).to(ty)
     mask = None
-    if with_mask:
+    if with_mask in NEG_INF_MASKS:
+        mask = neg_inf_mask(with_mask, Tq, Tk, ty)
+    elif with_mask:
         mask = torch.zeros(Tq, Tk, device="cuda", dtype=ty)
         mask[:, Tk // 3: Tk // 3 + 40] = -65504.0 if dtype == F16 else -3.0e38     # a band of padded positions
         mask[:, :5] = -1.5
@@ -715,16 +726,17 @@ def test_attention_decode_matches_fp64(K, heads, Tq, Tk, d, dv, group, with_mask
     out = torch.empty(heads, Tq, dv, device="cuda", dtype=ty)
     for rep in range(2):    # twice: the tickets must re-arm themselves
         out.zero_()
-        rc = K.osb_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr() if with_mask else None, out.data_ptr(), heads, Tq, Tk, d, dv,
+        rc = K.osb_attention(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr() if mask is not None else None, out.data_ptr(), heads, Tq, Tk, d, dv,
                              scale, 0, group, dtype, _stream())
         assert rc == 0
         torch.cuda.synchronize()
         kk = k.double().repeat_interleave(group, 0); vv = v.double().repeat_interleave(group, 0)
         s = q.double() @ kk.transpose(1, 2) * scale
-        if with_mask:
+        if mask is not None:
             s = s + mask.double()
         ref = torch.softmax(s, -1) @ vv
         tol = 2e-3 if dtype == F16 else 1e-5
+        assert bool(torch.isfinite(out).all())
         assert float((out.double() - ref).abs().max()) <= tol * max(1.0, float(ref.abs().max()))
 
 

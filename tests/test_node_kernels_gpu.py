@@ -107,12 +107,13 @@ def _softmax_fp32_bar(p, lgap, n, threads, fast_exp):
 
 def _softmax_check(got, logits32, dtype, n, threads, fast_exp, what):
     """got vs the fp64 softmax of the fp32 logits the kernel forms: fp32 error (above) plus, for fp16, one rounding of the result
-    (half an ulp: 2^-11 relative, 2^-25 absolute below the fp16 normal range)."""
+    (half an ulp: 2^-11 relative, 2^-25 absolute below the fp16 normal range).  A -inf logit must give 0 (its gap counts as 0 in the
+    bar, which leaves the bar of that element at 1e-38 / 2^-25)."""
     lg = logits32.astype(np.float64)
     mx = lg.max(-1, keepdims=True)
     e = np.exp(lg - mx)
     ref = e / e.sum(-1, keepdims=True)
-    rel = _softmax_fp32_bar(ref, mx - lg, n, threads, fast_exp)
+    rel = _softmax_fp32_bar(ref, np.where(np.isfinite(lg), mx - lg, 0.0), n, threads, fast_exp)
     tol = ref * rel + 1e-38
     if dtype == F16:
         tol = tol + ref * 2.0 ** -11 + 2.0 ** -25
@@ -137,16 +138,22 @@ def test_softmax(K, dtype, rows, cols):
 SCALE = 0.125     # a power of two: x * scale is exact in fp32, so the logit x * scale + mask is ONE rounding with or without an FMA
 
 
-def _mask_rows(mask_rows, cols, dtype, rng):
-    """mask row 0: a band of -65504 (fp16) / -3e38 (fp32); row 1: small finite values; row 2: every column masked with the same value."""
+def _mask_rows(mask_rows, cols, dtype, rng, neg_inf=False):
+    """mask row 0: a band of -65504 (fp16) / -3e38 (fp32); row 1: small finite values; row 2: every column masked with the same value.
+    neg_inf: -inf instead, over keys [0, 40) on row 0 and over every key but the last on row 2, so that every row keeps a finite key."""
     neg = -65504.0 if dtype == F16 else -3.0e38
     m = np.zeros((mask_rows, cols), np.float32)
-    m[0, cols // 3: cols // 3 + max(cols // 4, 1)] = neg
+    if neg_inf:
+        m[0, :min(40, cols - 1)] = -np.inf
+    else:
+        m[0, cols // 3: cols // 3 + max(cols // 4, 1)] = neg
     if mask_rows > 1:
         m[1, :5] = -1.5
         m[1] += rng.standard_normal(cols).astype(np.float32) * 0.25
     if mask_rows > 2:
-        m[2, :] = neg
+        m[2, :] = -np.inf if neg_inf else neg
+        if neg_inf:
+            m[2, -1] = 0.0
     return m.astype(NP[dtype])
 
 
@@ -166,15 +173,16 @@ SOFTMAX_LD_CASES = [
 
 
 @pytest.mark.parametrize("inplace", [False, True])
-@pytest.mark.parametrize("masked", [False, True])
+@pytest.mark.parametrize("masked", [False, True, "ninf"])
 @pytest.mark.parametrize("dtype", [F16, F32])
 @pytest.mark.parametrize("path,cols,ld,off", SOFTMAX_LD_CASES)
 def test_softmax_scaled_ld(K, path, cols, ld, off, dtype, masked, inplace):
     """osb_softmax_scaled_ld on each of its kernels (warp: ld <= 256, __expf, zero-filled pad columns; smem: 512 <= cols <= 12288,
     aligned, cols % vec == 0, __expf; generic: expf), out of place and in place (x == y, as the engine calls it), with a [3, cols] mask
-    broadcast over 7 rows (row r reads mask row r % 3): a masked band, small finite values, and a fully masked row.  Row 4 holds logits
-    near 125, which overflow expf unless the row maximum is subtracted.  Bar: _softmax_check on the fp32 logits (exact: SCALE is a
-    power of two); a row masked everywhere with -3e38 (fp32) must be exactly uniform; the pad columns must be exactly 0."""
+    broadcast over 7 rows (row r reads mask row r % 3): a masked band, small finite values, and a fully masked row ("ninf": -inf over
+    the leading 40 keys and a row whose only finite key is the last).  Row 4 holds logits near 125, which overflow expf unless the row
+    maximum is subtracted.  Bar: _softmax_check on the fp32 logits (exact: SCALE is a power of two); a row masked everywhere with -3e38
+    (fp32) must be exactly uniform; the pad columns must be exactly 0."""
     import torch
     rows, mask_rows = 7, 3
     rng = np.random.default_rng(cols * 3 + ld + off)
@@ -189,7 +197,7 @@ def test_softmax_scaled_ld(K, path, cols, ld, off, dtype, masked, inplace):
         ybuf = xbuf
     else:
         ybuf = _offset_view(rows * ld, dtype, off)
-    mask = _mask_rows(mask_rows, cols, dtype, rng) if masked else None
+    mask = _mask_rows(mask_rows, cols, dtype, rng, neg_inf=masked == "ninf") if masked else None
     tmask = torch.from_numpy(mask).cuda() if masked else None
     rc = K.osb_softmax_scaled_ld(xbuf.data_ptr(), ybuf.data_ptr(), dtype, rows, cols, ld, SCALE,
                                  tmask.data_ptr() if masked else None, mask_rows if masked else 0, _stream())
@@ -208,7 +216,7 @@ def test_softmax_scaled_ld(K, path, cols, ld, off, dtype, masked, inplace):
     _softmax_check(got[:, :cols], logits, dtype, cols, threads, fast, f"{path} softmax cols {cols} ld {ld}")
     if ld > cols:
         assert (got[:, cols:] == 0).all(), f"pad columns not zero-filled: {got[:, cols:]}"
-    if masked and dtype == F32:
+    if masked is True and dtype == F32:
         full = got[2::mask_rows, :cols]            # rows whose mask row masks every column with -3e38: the logits are all equal
         assert (full == np.float32(1.0) / np.float32(cols)).all(), "a fully masked row is not uniform"
 
@@ -222,8 +230,31 @@ def test_softmax_scaled_ld_refuses_long_padded_rows(K):
 # 2. osb_attention beyond decode: the rows kernel (attention_rows_kernel)
 # ============================================================================================================================
 
+NEG_INF_MASKS = ("ninf_lead40", "ninf_splits", "ninf_one_key")
+
+
+def neg_inf_mask(kind, Tq, Tk, ty):
+    """[Tq, Tk] additive mask holding -inf, as an fp32 -FLT_MAX mask or two added -65504 masks become in fp16 and as a left-padded
+    prompt masks the leading keys.  ninf_lead40: keys [0, 40); ninf_splits: keys [0, 128) and [256, 384), the first and the third
+    128-key split of the split-KV decode kernel; ninf_one_key: every key but the last.  The last 5 keys get -1.5 on top.  Every row
+    keeps at least one finite key, so the fp64 answer is finite."""
+    import torch
+    m = torch.zeros(Tq, Tk, dtype=torch.float64)
+    m[:, Tk - 5:] = -1.5
+    if kind == "ninf_lead40":
+        m[:, :40] = float("-inf")
+    elif kind == "ninf_splits":
+        m[:, :128] = float("-inf")
+        m[:, 256:384] = float("-inf")
+    else:
+        assert kind == "ninf_one_key", kind
+        m[:, :Tk - 1] = float("-inf")
+    assert bool(torch.isfinite(m).any(-1).all()), (kind, Tk)
+    return m.to(ty).cuda()
+
+
 ATTN_ROWS_CASES = [
-    # heads, Tq, Tk, d, dv, kv_group, k_transposed, mask, dtype
+    # heads, Tq, Tk, d, dv, kv_group, k_transposed, mask (True: finite block masks; or a NEG_INF_MASKS kind), dtype
     (4, 3, 20, 40, 40, 1, 1, False, F16),      # K stored [h, d, Tk], Tk < 32
     (4, 5, 77, 64, 64, 2, 1, True, F16),       # Tk not a multiple of 32, grouped KV
     (2, 9, 300, 80, 80, 1, 1, True, F32),
@@ -232,14 +263,26 @@ ATTN_ROWS_CASES = [
     (32, 130, 256, 64, 64, 8, 0, False, F32),
     (4, 20, 100, 40, 72, 2, 0, True, F16),     # dv != d, dv % 32 != 0
     (3, 24, 200, 48, 24, 3, 0, True, F32),
+    # -inf over a row's first 32-key block: the running maximum stays -inf through it
+    (4, 5, 77, 64, 64, 2, 1, "ninf_lead40", F16),
+    (4, 5, 77, 64, 64, 2, 1, "ninf_lead40", F32),
+    (4, 5, 77, 64, 64, 2, 0, "ninf_lead40", F16),
+    (4, 5, 77, 64, 64, 2, 0, "ninf_lead40", F32),
+    (2, 9, 400, 80, 80, 1, 1, "ninf_splits", F32),     # K^T at Tk >= 256
+    (2, 17, 400, 40, 72, 2, 1, "ninf_splits", F16),
+    (32, 160, 400, 64, 64, 4, 0, "ninf_splits", F16),  # heads * Tq > 4096
+    (4, 3, 20, 40, 40, 1, 1, "ninf_one_key", F16),     # the finite key inside the first block
+    (3, 24, 200, 48, 24, 3, 0, "ninf_one_key", F32),
+    (4, 20, 100, 40, 72, 2, 0, "ninf_one_key", F16),
 ]
 
 
 @pytest.mark.parametrize("heads,Tq,Tk,d,dv,group,kt,with_mask,dtype", ATTN_ROWS_CASES)
 def test_attention_rows_matches_fp64(K, heads, Tq, Tk, d, dv, group, kt, with_mask, dtype):
-    """osb_attention on the per-row online-softmax kernel against fp64 softmax(Q K^T s + mask) V.  The mask masks whole 32-key blocks
-    with a finite value (-65504 / -3e38): keys [0, 32) on even query rows -- the first block a row sees -- and keys [64, 96) everywhere;
-    the last 5 keys get -1.5.  Bars of test_attention_decode_matches_fp64: 2e-3 (fp16) / 1e-5 (fp32) of max(1, max|ref|)."""
+    """osb_attention on the per-row online-softmax kernel against fp64 softmax(Q K^T s + mask) V.  The finite mask masks whole 32-key
+    blocks with -65504 / -3e38: keys [0, 32) on even query rows -- the first block a row sees -- and keys [64, 96) everywhere; the last
+    5 keys get -1.5.  The -inf masks are those of neg_inf_mask.  Bars of test_attention_decode_matches_fp64: 2e-3 (fp16) / 1e-5 (fp32)
+    of max(1, max|ref|); every output finite."""
     import torch
     ty = _tdt(dtype)
     g = torch.Generator(device="cuda").manual_seed(heads * 1000 + Tq * 10 + Tk)
@@ -248,7 +291,9 @@ def test_attention_rows_matches_fp64(K, heads, Tq, Tk, d, dv, group, kt, with_ma
     v = torch.randn(heads // group, Tk, dv, device="cuda", generator=g).to(ty)
     kin = k.transpose(1, 2).contiguous() if kt else k
     mask = None
-    if with_mask:
+    if with_mask in NEG_INF_MASKS:
+        mask = neg_inf_mask(with_mask, Tq, Tk, ty)
+    elif with_mask:
         neg = -65504.0 if dtype == F16 else -3.0e38
         mask = torch.zeros(Tq, Tk, device="cuda", dtype=ty)
         mask[0::2, :32] = neg
@@ -256,18 +301,18 @@ def test_attention_rows_matches_fp64(K, heads, Tq, Tk, d, dv, group, kt, with_ma
         mask[:, Tk - 5:] = -1.5
     scale = 1.0 / d ** 0.5
     out = torch.full((heads, Tq, dv), float("nan"), device="cuda", dtype=ty)
-    rc = K.osb_attention(q.data_ptr(), kin.data_ptr(), v.data_ptr(), mask.data_ptr() if with_mask else None, out.data_ptr(),
+    rc = K.osb_attention(q.data_ptr(), kin.data_ptr(), v.data_ptr(), mask.data_ptr() if mask is not None else None, out.data_ptr(),
                          heads, Tq, Tk, d, dv, scale, kt, group, dtype, _stream())
     assert rc == 0
     torch.cuda.synchronize()
     kk = k.double().repeat_interleave(group, 0)
     vv = v.double().repeat_interleave(group, 0)
     s = q.double() @ kk.transpose(1, 2) * scale
-    if with_mask:
+    if mask is not None:
         s = s + mask.double()
     ref = torch.softmax(s, -1) @ vv
     tol = (2e-3 if dtype == F16 else 1e-5) * max(1.0, float(ref.abs().max()))
-    assert not torch.isnan(out).any()
+    assert bool(torch.isfinite(out).all()), f"{int((~torch.isfinite(out)).sum())} / {out.numel()} outputs not finite"
     err = float((out.double() - ref).abs().max())
     assert err <= tol, f"max err {err:.3g} > {tol:.3g}"
 

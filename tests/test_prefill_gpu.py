@@ -1,6 +1,7 @@
 """Prompt prefill: one Model::run over T new tokens with a KV cache (src/llm.cpp:472-480).
 
-GPU tests (gpu marker): the grouped-KV masked flash attention kernel (osb_sdpa_flash) against fp64 math, the emitted Llama prefill
+GPU tests (gpu marker): the grouped-KV masked flash attention kernel (osb_sdpa_flash) against fp64 math -- at every accepted head dim,
+with -inf masks, rows of very different scale, any scale and no mask -- and its launch refusals, the emitted Llama prefill
 graphs against the reference's own Model::run() (stored reference outputs under tests/golden/oracle, tests/util.py), the routing of
 the prefill attention onto the kernel, and a decode step fed with each side's prefill cache.  CPU tests (no marker): the fusion plan
 of a prefill graph, the unchanged decode model text, and the numpy restatement of the prefill graph (mask construction included)
@@ -66,6 +67,7 @@ def K(engine_lib):
     lib.osb_sdpa_flash.argtypes = [vp] * 5 + [i64] * 5 + [cf, vp]
     lib.osb_sdpa_flash_ok.argtypes = [i64] * 6 + [ctypes.c_int]
     lib.osb_rope.argtypes = [vp] * 4 + [ctypes.c_int, i64, i64, i64, vp]
+    lib.osb_launch_count.restype = ctypes.c_uint64
     return lib
 
 
@@ -75,11 +77,24 @@ def _stream():
 
 
 def _mask(kind, Tq, Tk, past):
-    """0 / -65504 additive mask [Tq, Tk] as the prefill graph builds it: keep[t, j] = (j <= past + t) * attention_mask[j]."""
+    """0 / -65504 additive mask [Tq, Tk] as the prefill graph builds it: keep[t, j] = (j <= past + t) * attention_mask[j].  The ninf_*
+    kinds put -inf on every masked key (an fp32 -FLT_MAX mask in fp16): ninf_lead40 also masks keys [0, 40) (a left-padded prompt),
+    ninf_splits keys [0, 128) and [256, 384), ninf_one_key leaves every third row its last causal key only."""
     import torch
     keep = (torch.arange(Tk)[None, :] <= past + torch.arange(Tq)[:, None]).double()
     if kind == "band":
         keep[:, 100:160] = 0                                  # padded positions inside the cache
+    elif kind == "ninf_lead40":
+        keep[:, :40] = 0
+    elif kind == "ninf_splits":
+        keep[:, :128] = 0
+        keep[:, 256:384] = 0
+    elif kind == "ninf_one_key":
+        for t in range(0, Tq, 3):
+            keep[t, :past + t] = 0
+    if kind.startswith("ninf"):
+        assert bool((keep.sum(-1) > 0).all()), kind         # every row keeps a finite key
+        return torch.where(keep > 0, 0.0, float("-inf")).half().cuda()
     m = (1 - keep) * -65504.0
     if kind == "full_rows":
         m[:, :7] = -1.5                                       # finite non-trivial values too
@@ -95,41 +110,137 @@ SDPA_CASES = [
     (8, 2, 17, 17, 64, "causal", 0),             # Tq just above the decode threshold
     (4, 1, 130, 131, 40, "causal", 1),           # ragged: partial query and key tiles, odd Tk, d < 64
     (2, 2, 64, 129, 128, "full_rows", 65),       # rows fully masked at -65504
+] + [(4, 2, 33, 70, d, "causal", 37) for d in range(8, 129, 8)]     # every accepted head dim on one ragged shape
+
+# -inf masks (fp16 kernel only: the fp32 kernel's own tests hold it to -inf and -FLT_MAX masks)
+SDPA_NEG_INF_CASES = [
+    (8, 2, 64, 300, 64, "ninf_lead40", 236),
+    (8, 2, 64, 500, 128, "ninf_splits", 436),
+    (4, 1, 40, 140, 40, "ninf_one_key", 100),
 ]
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("Hq,Hkv,Tq,Tk,d,kind,past", SDPA_CASES)
-def test_sdpa_flash_matches_fp64(K, Hq, Hkv, Tq, Tk, d, kind, past):
-    """softmax(Q K^T s + mask) V in fp64 on the fp16-rounded operands.  P is rounded to fp16 before the second MMA, so
-    |err| <= 2^-8 sum p|v| + 2^-9 |ref| + 1e-4 (the bar of test_flash_attention); a second launch gives the same bits."""
+def _inputs(Hq, Hkv, Tq, Tk, d, row_scales=False):
+    """q [Hq, Tq, d], k / v [Hkv, Tk, d] fp16.  row_scales: query rows spread over three decades (|q| stays below 1e3, well inside
+    fp16) and key rows whose norm grows along the sequence, so the rows' maxima keep moving to later key tiles."""
     import torch
     g = torch.Generator(device="cuda").manual_seed(Hq * 7919 + Tq * 31 + Tk + d)
-    G = Hq // Hkv
-    q = torch.randn(Hq, Tq, d, device="cuda", generator=g).half()
-    k = torch.randn(Hkv, Tk, d, device="cuda", generator=g).half()
-    v = torch.randn(Hkv, Tk, d, device="cuda", generator=g).half()
-    mask = _mask(kind, Tq, Tk, past)
-    scale = float(np.float32(1.0 / d ** 0.5))
-    assert K.osb_sdpa_flash_ok(Hq, Hkv, Tq, Tk, d, d, F16) == 1
-    outs = []
-    for _ in range(2):
-        o = torch.full((Hq, Tq, d), float("nan"), device="cuda", dtype=torch.half)
-        rc = K.osb_sdpa_flash(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr(), o.data_ptr(), Hq, Hkv, Tq, Tk, d, scale, _stream())
-        assert rc == 0
-        torch.cuda.synchronize()
-        outs.append(o)
-    assert torch.equal(outs[0], outs[1]), "second launch differs"
-    o = outs[0]
-    assert not torch.isnan(o).any()
+    q = torch.randn(Hq, Tq, d, device="cuda", generator=g)
+    k = torch.randn(Hkv, Tk, d, device="cuda", generator=g)
+    v = torch.randn(Hkv, Tk, d, device="cuda", generator=g)
+    if row_scales:
+        q *= torch.logspace(-1, 2, Tq, device="cuda")[torch.randperm(Tq, device="cuda", generator=g)].view(1, Tq, 1)
+        k *= torch.linspace(0.25, 2.0, Tk, device="cuda").view(1, Tk, 1)
+    return q.half(), k.half(), v.half()
+
+
+def _flash(K, q, k, v, mask, scale):
+    import torch
+    Hq, Tq, d = q.shape
+    Hkv, Tk, _ = k.shape
+    o = torch.full((Hq, Tq, d), float("nan"), device="cuda", dtype=torch.half)
+    rc = K.osb_sdpa_flash(q.data_ptr(), k.data_ptr(), v.data_ptr(), mask.data_ptr() if mask is not None else None, o.data_ptr(),
+                          Hq, Hkv, Tq, Tk, d, scale, _stream())
+    assert rc == 0
+    torch.cuda.synchronize()
+    return o
+
+
+def _check(o, q, k, v, mask, scale):
+    """softmax(Q K^T s + mask) V in fp64 on the fp16-rounded operands.  P is rounded to fp16 before the second MMA, so
+    |err| <= 2^-8 sum p|v| + 2^-9 |ref| + 1e-4 (the bar of test_flash_attention); every output finite."""
+    import torch
+    G = q.shape[0] // k.shape[0]
     kk = k.double().repeat_interleave(G, 0)
     vv = v.double().repeat_interleave(G, 0)
-    P = torch.softmax(q.double() @ kk.transpose(1, 2) * scale + mask.double(), dim=-1)
+    s = q.double() @ kk.transpose(1, 2) * scale
+    P = torch.softmax(s + mask.double() if mask is not None else s, dim=-1)
     ref = P @ vv
     absref = P @ vv.abs()
+    assert bool(torch.isfinite(o).all()), f"{int((~torch.isfinite(o)).sum())} / {o.numel()} outputs not finite"
     err = (o.double() - ref).abs()
     tol = absref * 2.0 ** -8 + ref.abs() * 2.0 ** -9 + 1e-4
     assert not (err > tol).any(), f"max err {float(err.max()):.4g}, ref max {float(ref.abs().max()):.4g}, bad {(err > tol).sum().item()}"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("Hq,Hkv,Tq,Tk,d,kind,past", SDPA_CASES + SDPA_NEG_INF_CASES)
+def test_sdpa_flash_matches_fp64(K, Hq, Hkv, Tq, Tk, d, kind, past):
+    """The bar of _check; a second launch gives the same bits."""
+    import torch
+    q, k, v = _inputs(Hq, Hkv, Tq, Tk, d)
+    mask = _mask(kind, Tq, Tk, past)
+    scale = float(np.float32(1.0 / d ** 0.5))
+    assert K.osb_sdpa_flash_ok(Hq, Hkv, Tq, Tk, d, d, F16) == 1
+    a = _flash(K, q, k, v, mask, scale)
+    b = _flash(K, q, k, v, mask, scale)
+    assert torch.equal(a, b), "second launch differs"
+    _check(a, q, k, v, mask, scale)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("Hq,Hkv,Tq,Tk,d,past", [(32, 4, 512, 512, 64, 0), (8, 2, 333, 777, 128, 444), (4, 4, 300, 300, 40, 0)])
+def test_sdpa_flash_running_max(K, Hq, Hkv, Tq, Tk, d, past):
+    """Rows of very different scale under a causal mask: a kernel that kept the first tile's maximum or skipped the rescaling of O fails."""
+    q, k, v = _inputs(Hq, Hkv, Tq, Tk, d, row_scales=True)
+    mask = _mask("causal", Tq, Tk, past)
+    scale = float(np.float32(1.0 / d ** 0.5))
+    _check(_flash(K, q, k, v, mask, scale), q, k, v, mask, scale)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("d", [64, 128])
+def test_sdpa_flash_leading_neg_inf_tiles(K, d):
+    """-inf over the first 192 keys of every row (whole key tiles) and on the causally masked keys, in rows that have finite keys later:
+    those tiles must leave the running maximum, the sums and O untouched instead of making them NaN."""
+    Hq, Hkv, Tq, Tk, past = 8, 2, 200, 456, 256
+    q, k, v = _inputs(Hq, Hkv, Tq, Tk, d)
+    scale = float(np.float32(1.0 / d ** 0.5))
+    mask = _mask("causal", Tq, Tk, past)
+    mask[mask < 0] = float("-inf")
+    mask[:, :192] = float("-inf")
+    _check(_flash(K, q, k, v, mask, scale), q, k, v, mask, scale)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("scale", [-0.125, 0.9, 1e-3])
+def test_sdpa_flash_any_scale(K, scale):
+    """Any finite scale, negative included: the running maximum is taken over the masked, scaled logits."""
+    Hq, Hkv, Tq, Tk, d = 8, 2, 130, 200, 64
+    q, k, v = _inputs(Hq, Hkv, Tq, Tk, d)
+    mask = _mask("causal", Tq, Tk, Tk - Tq)
+    _check(_flash(K, q, k, v, mask, scale), q, k, v, mask, scale)
+
+
+@pytest.mark.gpu
+def test_sdpa_flash_no_mask(K):
+    """A null mask is softmax(Q K^T * scale) V."""
+    Hq, Hkv, Tq, Tk, d = 4, 2, 100, 170, 64
+    q, k, v = _inputs(Hq, Hkv, Tq, Tk, d)
+    scale = float(np.float32(1.0 / d ** 0.5))
+    _check(_flash(K, q, k, v, None, scale), q, k, v, None, scale)
+
+
+@pytest.mark.gpu
+def test_sdpa_flash_refuses_misaligned_pointers(K):
+    """q / k / v / out off 16-byte alignment and a mask off 4-byte alignment are refused before anything is enqueued: the launch count
+    stays and the output stays as it was.  A mask 4 bytes past a 16-byte boundary is taken."""
+    import torch
+    Hq, Hkv, Tq, Tk, d = 4, 2, 64, 64, 64
+    buf = torch.zeros(Hq * Tq * d + 64, device="cuda", dtype=torch.half)
+    mask = torch.zeros(Tq * Tk + 8, device="cuda", dtype=torch.half)
+    out = torch.full((Hq * Tq * d + 16,), 7.0, device="cuda", dtype=torch.half)
+    p = buf.data_ptr()
+
+    def refused(qoff=0, koff=0, voff=0, ooff=0, moff=0):          # byte offsets
+        n0 = K.osb_launch_count()
+        rc = K.osb_sdpa_flash(p + qoff, p + koff, p + voff, mask.data_ptr() + moff, out.data_ptr() + ooff, Hq, Hkv, Tq, Tk, d, 0.125, _stream())
+        torch.cuda.synchronize()
+        return rc != 0 and K.osb_launch_count() == n0
+    assert refused(qoff=8) and refused(koff=8) and refused(voff=2) and refused(ooff=8)
+    assert refused(moff=2)
+    assert bool((out == 7.0).all())
+    assert not refused(moff=4)
 
 
 @pytest.mark.gpu
