@@ -2274,10 +2274,11 @@ void Engine::Impl::fused_swiglu(const Step& s)
 void Engine::Impl::fused_layernorm(const Step& s)
 {
     size_t i = s.first;
+    // the planner accepts any scalar exponent; only 2 is a LayerNorm: any other runs as the ops it is
+    if (scalar_of(in(i + 2, 1), E.m_ops[i + 2]) != 2.f) { exec_unfused(s); return; }
     Tensor x = to_plain(in(i, 0));
-    Tensor eps_t = in(i + 4, 1), gamma = in(i + 7, 1), beta = in(i + 8, 1), pw = in(i + 2, 1);
+    Tensor eps_t = in(i + 4, 1), gamma = in(i + 7, 1), beta = in(i + 8, 1);
     float eps = scalar_of(eps_t, E.m_ops[i + 4]);
-    if (scalar_of(pw, E.m_ops[i + 2]) != 2.f) fail(E.m_ops[i + 2], "LayerNorm pattern with exponent != 2 (not implemented).");
     if (gamma.type != x.type) gamma = convert(gamma, x.type);
     if (beta.type != x.type) beta = convert(beta, x.type);
     Tensor y = make(x.type, x.shape);
@@ -2328,7 +2329,10 @@ void Engine::Impl::fused_geglu(const Step& s)
         Tensor a = to_plain(in(mm, 0)), bias = in(mm + 1, (size_t)s.bias_in);
         const TensorRef& wr = E.m_ops[mm].in[1];
         const int64_t Kd = wr.shape[0], inner = wr.shape[1] / 2, M = !a.shape.empty() && a.shape.back() == Kd && Kd > 0 ? a.numel() / Kd : 0;
-        if (a.type == DType::f16 && E.gemm_impl != 1 && M > 0 && gate_ok((int64_t)a.shape.size(), wr.shape[1])) {
+        // not the two halves (or an unexpected constant): all ten ops by their own handlers, the bias Add included -- a bias in the GEMM
+        // epilogue would round once where the MatMul and the Add round twice
+        if (!gate_ok((int64_t)a.shape.size(), wr.shape[1])) { exec_unfused(s); return; }
+        if (a.type == DType::f16 && E.gemm_impl != 1 && M > 0) {
             Tensor w = in(mm, 1);
             if (w.type != a.type) w = convert(w, a.type);
             if (bias.type != a.type) bias = convert(bias, a.type);
