@@ -61,6 +61,15 @@ int osb_tc_conv_f32x(const void* x6, const void* w6, const void* bias_f32, const
 int osb_tc_gemm_f32x_f16w_ok(int64_t M, int64_t N, int64_t K, int64_t ldb);
 int osb_tc_gemm_f32x_f16w(const void* A_f32, const void* B_f16, int64_t ldb, void* C_f32, const void* bias_f32, const void* residual_f32, int64_t M, int64_t N,
                           int64_t K, void* planes, void* stream);
+/* fp32 Conv on an fp16 weight read as stored, the same five products: y [Ho, Wo, Cout] = conv(x [H, W, Cin], float(w)) + bias [Cout] + residual
+   [Ho, Wo, Cout], x / y / bias / residual fp32 NHWC, w the OHWI fp16 blob [Cout][kh][kw][Cin]; the padding and stride of osb_tc_conv_f32x.
+   Shapes: Cin % 8 == 0, Cin >= 16, stride 1 or 2, kh, kw <= 7, H W >= 64; any Cout, and any output size (an unsplit launch stores the fp32
+   output itself; a split-K launch, only where its partials fit the workspace, adds them up in the fp32 reduce).  planes: scratch of 6 H W Cin
+   bytes, 16-byte aligned, for the bf16 planes of x.  cudaErrorNotSupported (801), nothing launched: a shape outside the above, unaligned x / w
+   / planes (16 bytes), y / residual (8 bytes) or bias (4 bytes). */
+int osb_tc_conv_f32x_f16w_ok(int64_t H, int64_t W, int64_t Cin, int64_t Cout, int kh, int kw, int stride, int64_t Ho, int64_t Wo);
+int osb_tc_conv_f32x_f16w(const void* x_f32, const void* w_f16, const void* bias_f32, const void* residual_f32, void* y_f32, int64_t H, int64_t W, int64_t Cin,
+                          int64_t Cout, int kh, int kw, int stride, int pad_top, int pad_left, int64_t Ho, int64_t Wo, void* planes, void* stream);
 /* Concat of two tensors along one axis in one launch (src/onnxstream.cpp Concat branch, two inputs): outer slices of a_bytes / b_bytes each.
    cudaErrorNotSupported (801) unless both slice sizes and all three pointers are multiples of 16 bytes. */
 int osb_concat2(const void* a, const void* b, void* out, int64_t outer, int64_t a_bytes, int64_t b_bytes, void* stream);

@@ -433,6 +433,7 @@ struct Engine::Impl {
         return t;
     }
     std::map<std::pair<size_t, size_t>, Tensor> wcache;  // weights of the current step (shared by all batch items)
+    static constexpr size_t W_STORED = ~(size_t)0;        // wcache input slot of a conv weight kept as its stored fp16 blob (op_conv)
 
     bool next_is_sole_consumer(size_t step_idx, const std::string& name)
     {
@@ -751,26 +752,36 @@ void Engine::Impl::op_conv(size_t oi, const Tensor* residual, size_t out_op)
         throw std::runtime_error("XnnPack::convolution_nhwc_fp32: one or more arguments are invalid.");
 
     Tensor x = in(oi, 0);
-    auto wkey = std::make_pair(oi, (size_t)1);
-    Tensor w;
-    if (op.in[1].wtype != DType::none) {
-        auto it = wcache.find(wkey);
-        if (it != wcache.end()) w = it->second; else { w = get_weight(oi, 1, false, true); wcache[wkey] = w; }
-    } else fail(op, "dynamic convolution weights are not supported (not implemented).");
+    if (op.in[1].wtype == DType::none) fail(op, "dynamic convolution weights are not supported (not implemented).");
+    const std::vector<int64_t>& wshape = op.in[1].shape;     // OIHW; get_weight returns it as OHWI
     Tensor b; bool has_b = op.in.size() > 2 && op.in[2].present;
-    if (has_b) b = in(oi, 2);
 
     if (x.shape.size() == 3) x.shape.push_back(1);   // Conv1D: trailing unit dim (src/onnxstream.cpp:2919-2920)
-    if (x.shape.size() != 4 || w.shape.size() != 4) throw std::runtime_error("XnnPack::convolution_nhwc_fp32: one or more arguments are invalid.");
-    if (w.shape[1] != ks[0] || w.shape[2] != ks[1]) fail(op, "invalid shape of W or invalid kernel_shape (not implemented?).");
+    if (x.shape.size() != 4 || wshape.size() != 4) throw std::runtime_error("XnnPack::convolution_nhwc_fp32: one or more arguments are invalid.");
+    if (wshape[2] != ks[0] || wshape[3] != ks[1]) fail(op, "invalid shape of W or invalid kernel_shape (not implemented?).");
     x = to_nhwc(x);
-    int64_t H = x.shape[2], W = x.shape[3], Cin = x.shape[1], Cout = w.shape[0];
-    if (w.shape[3] != Cin) throw std::runtime_error("XnnPack::convolution: invalid size of W.");
+    int64_t H = x.shape[2], W = x.shape[3], Cin = x.shape[1], Cout = wshape[0];
+    if (wshape[1] != Cin) throw std::runtime_error("XnnPack::convolution: invalid size of W.");
     int kh = (int)ks[0], kw = (int)ks[1], stride = (int)strides[0];
     // padding re-symmetrisation (src/onnxstream.cpp:1315-1331)
     int64_t ph = pads[0] + pads[2], pw = pads[1] + pads[3];
     int pad_top = (int)(ph / 2), pad_left = (int)(pw / 2);
     int64_t Ho = (H + ph - kh) / stride + 1, Wo = (W + pw - kw) / stride + 1;
+
+    // fp32 arithmetic meeting an fp16 blob: the tensor-core conv reads the blob as stored (osb_tc_conv_f32x_f16w) -- no fp32 copy, no bf16x6
+    // expansion.  Its wcache entry has a key of its own, so the fp16 blob never stands in for the fp32 weight of the routes below.
+    // Shape rule (H100, DESIGN.md section 5): it takes outputs of 128 x 128 pixels and more, where it measured 1.17-6.6x the route below
+    // at every SD VAE decoder shape, and every output the expanded route cannot take; at 64 x 64 and below (the SD 1.5 UNet, the decoder's
+    // latent level) the expanded route measured faster on most shapes and keeps them.
+    const bool f16w = x.type == DType::f32 && op.in[1].wtype == DType::f16 && E.gemm_impl != 1 && osb_tc_conv_f32x_f16w_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo) &&
+                      (Ho * Wo >= 128 * 128 || !osb_tc_conv_f32x_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo));
+    auto wkey = std::make_pair(oi, f16w ? W_STORED : (size_t)1);
+    Tensor w;
+    {
+        auto it = wcache.find(wkey);
+        if (it != wcache.end()) w = it->second; else { w = get_weight(oi, 1, false, true, f16w); wcache[wkey] = w; }
+    }
+    if (has_b) b = in(oi, 2);
 
     Tensor y;
     if (x.type == DType::u8) {
@@ -808,7 +819,7 @@ void Engine::Impl::op_conv(size_t oi, const Tensor* residual, size_t out_op)
         ck(osb_conv2d_qu8((const uint8_t*)x.data(), (const uint8_t*)w.data(), b32 ? (const int32_t*)b32->ptr : nullptr, (uint8_t*)y.mdata(),
                           H, W, Cin, Cout, kh, kw, stride, pad_top, pad_left, Ho, Wo, x.zero_point, x.scale, w.zero_point, w.scale, ozp, oscale, st), "osb_conv2d_qu8");
     } else {
-        if (w.type != x.type) w = convert(w, x.type);
+        if (w.type != x.type && !f16w) w = convert(w, x.type);
         if (has_b && b.type != x.type) b = convert(b, x.type);
         y = make(x.type, { 1, Cout, Ho, Wo }, Layout::nhwc);
         Tensor rr;
@@ -825,7 +836,14 @@ void Engine::Impl::op_conv(size_t oi, const Tensor* residual, size_t out_op)
             if (gn_apply_ok(y, Cout, G)) gstats = gn_slot_ptr(gn_slot);
         }
         bool done = false;
-        if (x.type == DType::f32 && E.gemm_impl != 1 && osb_tc_conv_f32x_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo)) {
+        if (f16w) {
+            Tensor planes = make(DType::f16, { 3 * H * W * Cin });     // the bf16 planes of x (6 bytes per element)
+            const int rc = osb_tc_conv_f32x_f16w(x.data(), w.data(), has_b ? b.data() : nullptr, residual ? rr.data() : nullptr, y.mdata(), H, W, Cin, Cout, kh, kw,
+                                                 stride, pad_top, pad_left, Ho, Wo, planes.mdata(), st);
+            if (rc == (int)cudaErrorNotSupported) w = convert(w, x.type);     // an operand the kernel cannot address: the fp32 routes below
+            else { ck(rc, "osb_tc_conv_f32x_f16w"); done = true; }
+        }
+        if (!done && x.type == DType::f32 && E.gemm_impl != 1 && osb_tc_conv_f32x_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo)) {
             // fp32 conv on the tensor cores: image and OHWI weights as bf16 triple-split expansions (6 Cin channels), fp32 result
             Tensor x6 = f32x_operand(x, H * W, Cin, false, 0, "");
             Tensor w6 = f32x_operand(w, Cout * kh * kw, Cin, false, 1, op.in[1].name + "|bf16x6");

@@ -514,6 +514,13 @@ __global__ void splitk_reduce_f32_kernel(const float* __restrict__ ws, float* __
 //                     the fp32 accumulators, one stage in flight; the tile's raw fp32 sums go to the split-K workspace [split][M][N] and
 //                     splitk_reduce_f32_kernel adds the splits, fp32 bias and residual.
 // Each raw B block is converted once and its 16 KB read from L2 once; a stage is 48 KB of A planes + 32 KB of B parts, 2 stages.
+//
+// CONV (osb_tc_conv_f32x_f16w): the same pipeline as an implicit-GEMM convolution.  A is the NHWC image split into planes [H W][3][Cin],
+// read through a 4-D map (Cin, plane, W, H): plane p of k-block (tap, channel block) is one box of bh x bw pixels at the tap's offset,
+// zero-filled outside the image and past Cin (a 3-D map over 3 Cin channels would read the next plane there, against the next tap's
+// weights in B).  B is the OHWI fp16 blob [Cout][kh kw Cin] as stored, K-major, as the fp16 conv reads it.  An unsplit launch stores fp32
+// from the registers (acc + bias[n] + residual, the reduce kernel's order), so the output is not bounded by the workspace; a split
+// launch writes its partials to the workspace for splitk_reduce_f32_kernel.  Ragged Cout stores are guarded by column.
 namespace f16w {
 constexpr int A_PLANE_BYTES = BLOCK_M * BLOCK_K * 2;            // 16 KB
 constexpr int A_BYTES = 3 * A_PLANE_BYTES;
@@ -535,7 +542,9 @@ __device__ __forceinline__ void f16x2_bf16_parts(uint32_t v, uint32_t& hi, uint3
     lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
-// p: M, N, K, m_tiles, n_tiles, k_blocks_per_tap (= ceil(K / 64)), split_k, ws
+// p: M, N, K, m_tiles, n_tiles, k_blocks_per_tap (= ceil(K / 64)), split_k, ws; CONV also the conv geometry (K = Cin, M = Ho Wo, taps,
+// kw, pads, stride, bw x bh boxes, tiles_x) and, unsplit, C / bias / residual as fp32
+template <bool CONV>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const TcParams p)
 {
@@ -563,7 +572,7 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
 
     const int tiles = p.m_tiles * p.n_tiles;
     const int total = tiles * p.split_k;
-    const int kbk = p.k_blocks_per_tap;
+    const int kbk = CONV ? p.taps * p.k_blocks_per_tap : p.k_blocks_per_tap;
     const int kb_per_split = (kbk + p.split_k - 1) / p.split_k;   // host guarantees every split runs >= 1 k-block
 
     if (warp == 0) {
@@ -574,18 +583,35 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
             const int sp = tile % p.split_k, r = tile / p.split_k;
             const int m0 = (r % p.m_tiles) * BLOCK_M, n0 = (r / p.m_tiles) * BLOCK_N;
             const int kb_lo = sp * kb_per_split, kb_hi = min(kb_lo + kb_per_split, kbk);
+            // CONV: the box origin of the tile's pixels and the (tap, channel block) walk, incremental inside the k loop
+            int tap = 0, kcb = 0, ky = 0, kx = 0, ax = 0, ay = 0;
+            if constexpr (CONV) {
+                const int mt = r % p.m_tiles;
+                ax = (mt % p.tiles_x) * p.bw * p.stride - p.pad_left; ay = (mt / p.tiles_x) * p.bh * p.stride - p.pad_top;
+                tap = kb_lo / p.k_blocks_per_tap; kcb = kb_lo % p.k_blocks_per_tap; ky = tap / p.kw; kx = tap % p.kw;
+            }
             for (int kb = kb_lo; kb < kb_hi; kb++) {
                 mbar_wait(&empty[stage], phase ^ 1);
                 if (elect_one()) {
                     mbar_expect_tx(&landed[stage], A_BYTES + B_PART_BYTES);
-                    const int kc = kb * BLOCK_K;
                     const uint32_t sa = sa0 + stage * A_BYTES, sb = sb0 + stage * B_BYTES;
+                    if constexpr (CONV) {
+                        const int kc = kcb * BLOCK_K;
 #pragma unroll
-                    for (int pl = 0; pl < 3; pl++) tma_load_3d_s(sa + pl * A_PLANE_BYTES, &map_a, &landed[stage], pl * p.K + kc, m0, 0);
+                        for (int pl = 0; pl < 3; pl++) tma_load_4d_s(sa + pl * A_PLANE_BYTES, &map_a, &landed[stage], kc, pl, ax + kx, ay + ky);
+                        tma_load_3d_s(sb, &map_b, &landed[stage], tap * p.K + kc, n0, 0);
+                    } else {
+                        const int kc = kb * BLOCK_K;
 #pragma unroll
-                    for (int at = 0; at < 2; at++) tma_load_3d_s(sb + at * 8192, &map_b, &landed[stage], n0 + 64 * at, kc, 0);
+                        for (int pl = 0; pl < 3; pl++) tma_load_3d_s(sa + pl * A_PLANE_BYTES, &map_a, &landed[stage], pl * p.K + kc, m0, 0);
+#pragma unroll
+                        for (int at = 0; at < 2; at++) tma_load_3d_s(sb + at * 8192, &map_b, &landed[stage], n0 + 64 * at, kc, 0);
+                    }
                 }
                 __syncwarp();
+                if constexpr (CONV) {
+                    if (++kcb == p.k_blocks_per_tap) { kcb = 0; tap++; if (++kx == p.kw) { kx = 0; ky++; } }
+                }
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
         }
@@ -624,7 +650,9 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
         // ===================== consumers: 5 products per stage, fp32 partials out =====================
         const int wg = (warp >> 2) - 1;
         const uint64_t adesc0 = make_smem_desc(smem_u32(smem_a) + 64 * wg * 128, 16, 1024);
-        const uint64_t bdesc0 = make_smem_desc(smem_u32(smem_b), 8192, 1024);
+        // B: MN-major (GEMM: [K][N] weight, two 64-column atoms) or K-major (CONV: 128 OHWI rows of 64 k)
+        const uint64_t bdesc0 = CONV ? make_smem_desc(smem_u32(smem_b), 16, 1024) : make_smem_desc(smem_u32(smem_b), 8192, 1024);
+        constexpr uint32_t b_kstep = CONV ? (WG_K * 2) >> 4 : (WG_K * 128) >> 4;
         constexpr uint64_t AP = A_PLANE_BYTES >> 4, BP = B_PART_BYTES >> 4;   // descriptor units (16 B)
         const int r_lo = 64 * wg + (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
         const bool pair_ok = (p.N & 1) == 0;
@@ -647,7 +675,7 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
                 for (int x = 0; x < 5; x++) {
 #pragma unroll
                     for (int k = 0; k < BLOCK_K / WG_K; k++)
-                        wgmma_ss<128, 1, true>(acc, ad[x] + (uint64_t)(k * ((WG_K * 2) >> 4)), bd[x] + (uint64_t)(k * ((WG_K * 128) >> 4)), 1u);
+                        wgmma_ss<128, CONV ? 0 : 1, true>(acc, ad[x] + (uint64_t)(k * ((WG_K * 2) >> 4)), bd[x] + (uint64_t)(k * b_kstep), 1u);
                 }
                 wgmma_commit();
                 if (prev >= 0) { wgmma_wait<1>(); mbar_arrive(&empty[prev]); }
@@ -656,18 +684,48 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
             }
             wgmma_wait<0>();
             mbar_arrive(&empty[prev]);
-            // raw fp32 sums of this split -> ws[sp][M][N]
+            if constexpr (CONV) {
+                // the tile's rows are a bw x bh box of output pixels
+                const int mt = r % p.m_tiles, ty = (mt / p.tiles_x) * p.bh, tx = (mt % p.tiles_x) * p.bw;
+                const float* bias = reinterpret_cast<const float*>(p.bias);
+                const float* res = reinterpret_cast<const float*>(p.residual);
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int m = m0 + r_lo + 8 * h;
-                if (m >= p.M) continue;
-                float* wrow = p.ws + ((long long)sp * p.M + m) * p.N;
+                for (int h = 0; h < 2; h++) {
+                    const int rt = r_lo + 8 * h, y = ty + rt / p.bw, x = tx + rt % p.bw;
+                    if (y >= p.Ho || x >= p.Wo) continue;
+                    const long long row = (long long)y * p.Wo + x;
+                    // split: raw partials -> ws[sp][M][N]; unsplit: acc + bias + residual -> C, fp32
+                    float* out = p.split_k > 1 ? p.ws + ((long long)sp * p.M + row) * p.N : reinterpret_cast<float*>(p.C) + row * p.N;
+                    const float* rrow = p.split_k > 1 || !res ? nullptr : res + row * p.N;
+                    const float* b = p.split_k > 1 ? nullptr : bias;
 #pragma unroll
-                for (int j = 0; j < 16; j++) {
-                    const int n = n0 + 8 * j + cq;
-                    const float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-                    if (n + 1 < p.N && pair_ok) *reinterpret_cast<float2*>(wrow + n) = make_float2(f0, f1);
-                    else { if (n < p.N) wrow[n] = f0; if (n + 1 < p.N) wrow[n + 1] = f1; }
+                    for (int j = 0; j < 16; j++) {
+                        const int n = n0 + 8 * j + cq;
+                        const bool ok0 = n < p.N, ok1 = n + 1 < p.N;
+                        float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                        if (b) { if (ok0) f0 += b[n]; if (ok1) f1 += b[n + 1]; }
+                        if (rrow) {
+                            if (ok1 && pair_ok) { const float2 rv = *reinterpret_cast<const float2*>(rrow + n); f0 += rv.x; f1 += rv.y; }
+                            else { if (ok0) f0 += rrow[n]; if (ok1) f1 += rrow[n + 1]; }
+                        }
+                        if (ok1 && pair_ok) *reinterpret_cast<float2*>(out + n) = make_float2(f0, f1);
+                        else { if (ok0) out[n] = f0; if (ok1) out[n + 1] = f1; }
+                    }
+                }
+            } else {
+                // raw fp32 sums of this split -> ws[sp][M][N]
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const int m = m0 + r_lo + 8 * h;
+                    if (m >= p.M) continue;
+                    float* wrow = p.ws + ((long long)sp * p.M + m) * p.N;
+#pragma unroll
+                    for (int j = 0; j < 16; j++) {
+                        const int n = n0 + 8 * j + cq;
+                        const float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                        if (n + 1 < p.N && pair_ok) *reinterpret_cast<float2*>(wrow + n) = make_float2(f0, f1);
+                        else { if (n < p.N) wrow[n] = f0; if (n + 1 < p.N) wrow[n + 1] = f1; }
+                    }
                 }
             }
         }
@@ -1385,7 +1443,7 @@ extern "C" int osb_tc_gemm_f32x_f16w(const void* A, const void* B, int64_t ldb, 
         if (!make_map_rb(&ma[i], pl + m0 * K3, (uint64_t)K3, (uint64_t)rows, 1, (uint64_t)K3 * 2, (uint64_t)(rows * K3) * 2, BLOCK_K, BLOCK_M, &sw))
             return (int)cudaErrorNotSupported;
     }
-    static const cudaError_t attr = cudaFuncSetAttribute(tc_gemm_f16w_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, f16w::SMEM_BYTES);
+    static const cudaError_t attr = cudaFuncSetAttribute(tc_gemm_f16w_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, f16w::SMEM_BYTES);
     if (attr != cudaSuccess) return (int)attr;
     int e = osb_f32x_split_rows((const float*)A, (__nv_bfloat16*)planes, M, K, st);
     if (e) return e;
@@ -1400,7 +1458,7 @@ extern "C" int osb_tc_gemm_f32x_f16w(const void* A, const void* B, int64_t ldb, 
         if ((size_t)p.split_k * rows * N * 4 > WS_MAX) p.split_k = 1;
         p.ws = wsp->splitk;
         const int grid = (int)std::min<int64_t>((int64_t)p.m_tiles * p.n_tiles * p.split_k, num_sms());
-        osb_launch((tc_gemm_f16w_kernel), grid, NUM_THREADS, (size_t)f16w::SMEM_BYTES, st, ma[i], mb, p);
+        osb_launch((tc_gemm_f16w_kernel<false>), grid, NUM_THREADS, (size_t)f16w::SMEM_BYTES, st, ma[i], mb, p);
         if ((e = launched(1))) return e;
         const long long total = rows * N;
         osb_launch((splitk_reduce_f32_kernel), (int)std::min<long long>((total + 255) / 256, num_sms() * 8), 256, 0, st, (const float*)p.ws,
@@ -1408,4 +1466,69 @@ extern "C" int osb_tc_gemm_f32x_f16w(const void* A, const void* B, int64_t ldb, 
         if ((e = launched())) return e;
     }
     return 0;
+}
+
+// ---- fp32 conv on an fp16 weight read in place ------------------------------------------------------------------------------------------
+// The shapes of osb_tc_conv_ok; the output is stored from the registers, so its size is not bounded by the workspace.
+extern "C" int osb_tc_conv_f32x_f16w_ok(int64_t H, int64_t W, int64_t Cin, int64_t Cout, int kh, int kw, int stride, int64_t Ho, int64_t Wo)
+{
+    return f32_tc_on() && Cout >= 1 && kh >= 1 && kw >= 1 && Ho >= 1 && Wo >= 1 && Ho * Wo <= (1 << 30) && Cout <= (1 << 30) &&
+           (int64_t)kh * kw * Cin <= (1 << 30) && osb_tc_conv_ok(H, W, Cin, Cout, kh, kw, stride, nullptr, nullptr, nullptr) ? 1 : 0;
+}
+
+// y [Ho, Wo, Cout] fp32 = conv(x [H, W, Cin] fp32, float(w) [Cout][kh][kw][Cin] fp16) + bias [Cout] + residual [Ho, Wo, Cout] (fp32, either may
+// be null): the split of x into `planes`, tc_gemm_f16w_kernel<true>, and the fp32 reduce when the launch splits K.
+extern "C" int osb_tc_conv_f32x_f16w(const void* x, const void* w, const void* bias, const void* residual, void* y, int64_t H, int64_t W, int64_t Cin,
+                                     int64_t Cout, int kh, int kw, int stride, int pad_top, int pad_left, int64_t Ho, int64_t Wo, void* planes, void* stream)
+{
+    if (!osb_tc_conv_f32x_f16w_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo) || !aligned16(x) || !aligned16(w) || !aligned16(planes) || ((uintptr_t)y & 7) ||
+        ((uintptr_t)bias & 3) || ((uintptr_t)residual & 7))
+        return (int)cudaErrorNotSupported;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int kbpt = (int)((Cin + BLOCK_K - 1) / BLOCK_K), k_blocks = kh * kw * kbpt;
+    const int64_t M = Ho * Wo;
+    // the fp32 path's split rule (old_split) over the raw k-blocks, each five products deep; osb_tc_set_tile's forced split, clamped so
+    // that no split is empty.  A split runs only where its partials fit the workspace; unsplit, the kernel stores the output itself.
+    int split = choose_tile(TileProblem{ (int)M, (int)Cout, (int)Ho, (int)Wo, 1, 1, k_blocks, 1, true, true }).split;
+    if (g_tile_split > 0) {
+        split = std::min(g_tile_split, k_blocks);
+        if (split > 1) { const int kb_per = (k_blocks + split - 1) / split; split = (k_blocks + kb_per - 1) / kb_per; }
+    }
+    if ((size_t)split * M * Cout * 4 > WS_MAX) split = 1;
+    OsbWorkspace* wsp = split > 1 ? osb_workspace(st, OSB_WS_SPLITK) : nullptr;
+    if (!wsp) split = 1;
+    const uint32_t bw = (uint32_t)conv_box_w(BLOCK_M, (int)Wo), bh = BLOCK_M / bw;
+    CUtensorMap ma, mb;
+    // A: the planes [H][W][3][Cin] as (Cin, plane, W, H); one box = one plane of bh rows x bw pixels x 64 channels
+    if (!make_map_4d(&ma, planes, (uint64_t)Cin, 3, (uint64_t)W, (uint64_t)H, (uint64_t)Cin * 2, (uint64_t)Cin * 6, (uint64_t)W * Cin * 6, BLOCK_K, 1,
+                     bw * stride, bh * stride, (uint32_t)stride))
+        return (int)cudaErrorNotSupported;
+    // B: OHWI weights = [Cout][kh*kw*Cin], K-major
+    const int64_t Ktot = (int64_t)kh * kw * Cin;
+    if (!make_map(&mb, w, (uint64_t)Ktot, (uint64_t)Cout, 1, (uint64_t)Ktot * 2, (uint64_t)Ktot * Cout * 2, BLOCK_K, BLOCK_N, 1)) return (int)cudaErrorNotSupported;
+    static const cudaError_t attr = cudaFuncSetAttribute(tc_gemm_f16w_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, f16w::SMEM_BYTES);
+    if (attr != cudaSuccess) return (int)attr;
+    TcParams p{};
+    p.M = (int)M; p.N = (int)Cout; p.K = (int)Cin; p.batch = 1;
+    p.bm = BLOCK_M; p.bn = BLOCK_N;
+    p.tiles_x = (int)((Wo + bw - 1) / bw);
+    p.m_tiles = p.tiles_x * (int)((Ho + bh - 1) / bh);
+    p.n_tiles = (int)((Cout + BLOCK_N - 1) / BLOCK_N);
+    p.b_kmajor = 1;
+    p.taps = kh * kw; p.kw = kw; p.pad_top = pad_top; p.pad_left = pad_left; p.Wo = (int)Wo; p.Ho = (int)Ho; p.bw = (int)bw; p.bh = (int)bh;
+    p.k_blocks_per_tap = kbpt;
+    p.stride = stride;
+    p.C = (__half*)y; p.bias = (const __half*)bias; p.residual = (const __half*)residual; p.ldc = Cout;   // fp32 (see the kernel)
+    p.split_k = split;
+    p.ws = wsp ? wsp->splitk : nullptr;
+    int e = osb_f32x_split_rows((const float*)x, (__nv_bfloat16*)planes, H * W, Cin, st);
+    if (e) return e;
+    const int grid = (int)std::min<int64_t>((int64_t)p.m_tiles * p.n_tiles * split, num_sms());
+    osb_launch((tc_gemm_f16w_kernel<true>), grid, NUM_THREADS, (size_t)f16w::SMEM_BYTES, st, ma, mb, p);
+    if ((e = launched(1))) return e;
+    if (split == 1) return 0;
+    const long long total = M * Cout;
+    osb_launch((splitk_reduce_f32_kernel), (int)std::min<long long>((total + 255) / 256, num_sms() * 8), 256, 0, st, (const float*)p.ws, (float*)y,
+               (const float*)bias, (const float*)residual, (long long)M, (int)Cout, split);
+    return launched();
 }

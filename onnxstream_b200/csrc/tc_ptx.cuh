@@ -41,6 +41,22 @@ inline bool make_map(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d
     return r == CUDA_SUCCESS;
 }
 
+// rank-4 bf16 tensor map with 128B swizzle; dims/strides innermost first, traversal strides (1, 1, s, s) (the bf16 planes of an NHWC
+// image as (C, plane, W, H): a strided conv takes every s-th pixel of the box span)
+inline bool make_map_4d(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3, uint64_t s1_bytes, uint64_t s2_bytes,
+                        uint64_t s3_bytes, uint32_t b0, uint32_t b1, uint32_t b2, uint32_t b3, uint32_t traversal_stride)
+{
+    auto enc = get_encode();
+    if (!enc) return false;
+    cuuint64_t dims[4] = { d0, d1, d2, d3 };
+    cuuint64_t strides[3] = { s1_bytes, s2_bytes, s3_bytes };
+    cuuint32_t box[4] = { b0, b1, b2, b3 };
+    cuuint32_t estr[4] = { 1, 1, traversal_stride, traversal_stride };
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
+
 // ---- PTX wrappers ---------------------------------------------------------------------------------------------
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -89,6 +105,11 @@ __device__ __forceinline__ void tma_load_3d_s(uint32_t smem_addr, const CUtensor
 {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_addr), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void tma_load_4d_s(uint32_t smem_addr, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3)
+{
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+                 ::"r"(smem_addr), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 // TMA multicast: the box lands at the same shared-memory offset in every CTA of `cta_mask` and completes bytes on the mbarrier at the
 // same offset in each of them
