@@ -70,6 +70,20 @@ int osb_tc_gemm_f32x_f16w(const void* A_f32, const void* B_f16, int64_t ldb, voi
 int osb_tc_conv_f32x_f16w_ok(int64_t H, int64_t W, int64_t Cin, int64_t Cout, int kh, int kw, int stride, int64_t Ho, int64_t Wo);
 int osb_tc_conv_f32x_f16w(const void* x_f32, const void* w_f16, const void* bias_f32, const void* residual_f32, void* y_f32, int64_t H, int64_t W, int64_t Cin,
                           int64_t Cout, int kh, int kw, int stride, int pad_top, int pad_left, int64_t Ho, int64_t Wo, void* planes, void* stream);
+/* fp32 MatMul / Conv on a uint8 weight read as stored (W8A32): the weight is (q - zero_point) * scale with q the uint8 blob.  q - z is exact as
+   one bf16, so x (q - z) is three exact products of the bf16 planes of x; the scale is applied once, in fp32, in the epilogue: out =
+   acc * scale + bias + residual.  Otherwise shaped like the _f16w twins above: B [K, N] uint8 with rows ldb elements apart (GEMM), w the OHWI
+   uint8 blob [Cout][kh][kw][Cin] (conv); planes as there.  An unsplit launch stores the fp32 output itself, so neither output is bounded by
+   the workspace.  cudaErrorNotSupported (801), nothing launched: K % 8, ldb % 16, ldb < N (GEMM); a conv shape the _f16w conv refuses or
+   kh kw Cin % 16 (conv); a zero point outside [0, 255]; unaligned A / x / B / w / planes (16 bytes), C / y / residual (8 bytes) or bias
+   (4 bytes). */
+int osb_tc_gemm_f32x_u8w_ok(int64_t M, int64_t N, int64_t K, int64_t ldb, int zero_point);
+int osb_tc_gemm_f32x_u8w(const void* A_f32, const void* B_u8, int64_t ldb, void* C_f32, const void* bias_f32, const void* residual_f32, int64_t M, int64_t N,
+                         int64_t K, float scale, int zero_point, void* planes, void* stream);
+int osb_tc_conv_f32x_u8w_ok(int64_t H, int64_t W, int64_t Cin, int64_t Cout, int kh, int kw, int stride, int64_t Ho, int64_t Wo, int zero_point);
+int osb_tc_conv_f32x_u8w(const void* x_f32, const void* w_u8, const void* bias_f32, const void* residual_f32, void* y_f32, int64_t H, int64_t W, int64_t Cin,
+                         int64_t Cout, int kh, int kw, int stride, int pad_top, int pad_left, int64_t Ho, int64_t Wo, float scale, int zero_point, void* planes,
+                         void* stream);
 /* Concat of two tensors along one axis in one launch (src/onnxstream.cpp Concat branch, two inputs): outer slices of a_bytes / b_bytes each.
    cudaErrorNotSupported (801) unless both slice sizes and all three pointers are multiples of 16 bytes. */
 int osb_concat2(const void* a, const void* b, void* out, int64_t outer, int64_t a_bytes, int64_t b_bytes, void* stream);

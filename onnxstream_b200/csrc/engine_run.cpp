@@ -217,6 +217,33 @@ struct Engine::Impl {
     bool f16w_gemm(const OpDef& op, const Tensor& a) const { return f16w_rows(op, a) > 8 && E.gemm_impl != 1; }
     bool f16w_gemm_run(size_t oi, const Tensor& a, const Tensor* bias, const Tensor* residual, size_t out_oi);
 
+    // W8A32: fp32 arithmetic meeting a static uint8 weight (scale, zero point).  The tensor-core GEMM and conv read the blob as stored and
+    // apply the scale in their epilogue (osb_tc_gemm_f32x_u8w, osb_tc_conv_f32x_u8w): no fp32 copy of the weight, no bf16x6 expansion.
+    // Not under uint8 arithmetic or QDQ, not under fp16 arithmetic (W8A16 keeps its route), not with the CUDA-core GEMM (b200_gemm_impl = 1);
+    // OSB_W8A32_TC=0 turns it off, so the fp32-copy route can be timed against it.
+    bool u8w_weight(const OpDef& op) const
+    {
+        static const bool on = [] { const char* e = getenv("OSB_W8A32_TC"); return !(e && e[0] == '0'); }();
+        const TensorRef& wr = op.in[1];
+        return on && wr.wtype == DType::u8 && !E.use_uint8_arithmetic && !E.use_uint8_qdq && !E.use_fp16_arithmetic && E.gemm_impl != 1;
+    }
+    // a MatMul / Gemm with more than 2 activation rows on a 2-D uint8 weight (at 2 rows or fewer the uint8 GEMV stays first)
+    bool u8w_gemm(const OpDef& op, const Tensor& a) const
+    {
+        const TensorRef& wr = op.in[1];
+        if (a.type != DType::f32 || !u8w_weight(op) || wr.shape.size() != 2 || a.shape.empty() || a.shape.back() != wr.shape[0]) return false;
+        return a.numel() / wr.shape[0] > 2 && osb_tc_gemm_f32x_u8w_ok(a.numel() / wr.shape[0], wr.shape[1], wr.shape[0], wr.shape[1], wr.zero_point);
+    }
+    bool u8w_gemm_run(size_t oi, const Tensor& a, const Tensor* bias, const Tensor* residual, size_t out_oi);
+    // the q, k and v projections of the fused attention block at op i all on uint8 weights (mha_project)
+    bool mha_u8w(size_t i, DType ty) const
+    {
+        for (size_t k : { (size_t)0, (size_t)4, (size_t)9 })
+            if (E.m_ops[i + k].in[1].shape.size() != 2 || !u8w_weight(E.m_ops[i + k])) return false;
+        return ty == DType::f32;
+    }
+    void u8w_project(size_t oi, const Tensor& x, int64_t rows, Tensor& out);
+
     DType act_dtype() const { return E.use_fp16_arithmetic ? DType::f16 : DType::f32; }
 
     // ------------------------------------------------------------------------------------------------------
@@ -433,7 +460,7 @@ struct Engine::Impl {
         return t;
     }
     std::map<std::pair<size_t, size_t>, Tensor> wcache;  // weights of the current step (shared by all batch items)
-    static constexpr size_t W_STORED = ~(size_t)0;        // wcache input slot of a conv weight kept as its stored fp16 blob (op_conv)
+    static constexpr size_t W_STORED = ~(size_t)0;        // wcache input slot of a conv weight kept as its stored fp16 / uint8 blob (op_conv)
 
     bool next_is_sole_consumer(size_t step_idx, const std::string& name)
     {
@@ -775,11 +802,13 @@ void Engine::Impl::op_conv(size_t oi, const Tensor* residual, size_t out_op)
     // latent level) the expanded route measured faster on most shapes and keeps them.
     const bool f16w = x.type == DType::f32 && op.in[1].wtype == DType::f16 && E.gemm_impl != 1 && osb_tc_conv_f32x_f16w_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo) &&
                       (Ho * Wo >= 128 * 128 || !osb_tc_conv_f32x_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo));
-    auto wkey = std::make_pair(oi, f16w ? W_STORED : (size_t)1);
+    // W8A32 (u8w_weight): the tensor-core conv reads the uint8 blob as stored (osb_tc_conv_f32x_u8w), under the same key of its own
+    const bool u8w = x.type == DType::f32 && u8w_weight(op) && osb_tc_conv_f32x_u8w_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo, op.in[1].zero_point);
+    auto wkey = std::make_pair(oi, f16w || u8w ? W_STORED : (size_t)1);
     Tensor w;
     {
         auto it = wcache.find(wkey);
-        if (it != wcache.end()) w = it->second; else { w = get_weight(oi, 1, false, true, f16w); wcache[wkey] = w; }
+        if (it != wcache.end()) w = it->second; else { w = get_weight(oi, 1, false, true, f16w || u8w); wcache[wkey] = w; }
     }
     if (has_b) b = in(oi, 2);
 
@@ -819,7 +848,7 @@ void Engine::Impl::op_conv(size_t oi, const Tensor* residual, size_t out_op)
         ck(osb_conv2d_qu8((const uint8_t*)x.data(), (const uint8_t*)w.data(), b32 ? (const int32_t*)b32->ptr : nullptr, (uint8_t*)y.mdata(),
                           H, W, Cin, Cout, kh, kw, stride, pad_top, pad_left, Ho, Wo, x.zero_point, x.scale, w.zero_point, w.scale, ozp, oscale, st), "osb_conv2d_qu8");
     } else {
-        if (w.type != x.type && !f16w) w = convert(w, x.type);
+        if (w.type != x.type && !f16w && !u8w) w = convert(w, x.type);
         if (has_b && b.type != x.type) b = convert(b, x.type);
         y = make(x.type, { 1, Cout, Ho, Wo }, Layout::nhwc);
         Tensor rr;
@@ -842,6 +871,13 @@ void Engine::Impl::op_conv(size_t oi, const Tensor* residual, size_t out_op)
                                                  stride, pad_top, pad_left, Ho, Wo, planes.mdata(), st);
             if (rc == (int)cudaErrorNotSupported) w = convert(w, x.type);     // an operand the kernel cannot address: the fp32 routes below
             else { ck(rc, "osb_tc_conv_f32x_f16w"); done = true; }
+        }
+        if (u8w) {
+            Tensor planes = make(DType::f16, { 3 * H * W * Cin });     // the bf16 planes of x (6 bytes per element)
+            const int rc = osb_tc_conv_f32x_u8w(x.data(), w.data(), has_b ? b.data() : nullptr, residual ? rr.data() : nullptr, y.mdata(), H, W, Cin, Cout, kh, kw,
+                                                stride, pad_top, pad_left, Ho, Wo, w.scale, w.zero_point, planes.mdata(), st);
+            if (rc == (int)cudaErrorNotSupported) w = convert(w, x.type);     // an operand the kernel cannot address: the fp32 routes below
+            else { ck(rc, "osb_tc_conv_f32x_u8w"); done = true; }
         }
         if (!done && x.type == DType::f32 && E.gemm_impl != 1 && osb_tc_conv_f32x_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo)) {
             // fp32 conv on the tensor cores: image and OHWI weights as bf16 triple-split expansions (6 Cin channels), fp32 result
@@ -911,6 +947,7 @@ void Engine::Impl::op_matmul(size_t oi, const Tensor* bias, const Tensor* residu
         if (rc != (int)cudaErrorNotSupported) ck(rc, "osb_gemv_f16w");
     }
     if (f16w_gemm(op, a) && f16w_gemm_run(oi, a, bias, residual, out_op == (size_t)-1 ? oi : out_op)) return;
+    if (u8w_gemm(op, a) && u8w_gemm_run(oi, a, bias, residual, out_op == (size_t)-1 ? oi : out_op)) return;
     Tensor b = to_plain(in(oi, 1));
     std::vector<int64_t> as = a.shape, bs = b.shape;
     bool lead1 = false, first2d = false;
@@ -1003,6 +1040,45 @@ bool Engine::Impl::f16w_gemm_run(size_t oi, const Tensor& a, const Tensor* bias,
     return true;
 }
 
+// A MatMul / Gemm on a uint8 blob under fp32 arithmetic (u8w_gemm): the tensor-core GEMM that reads the blob as stored -- streamed, the ring
+// slot; resident, the uint8 cache entry -- and caches no fp32 or expanded copy.  false = osb_tc_gemm_f32x_u8w refused: nothing pushed, the
+// caller takes its fp32 route.
+bool Engine::Impl::u8w_gemm_run(size_t oi, const Tensor& a, const Tensor* bias, const Tensor* residual, size_t out_oi)
+{
+    const TensorRef& wr = E.m_ops[oi].in[1];
+    const int64_t Kd = wr.shape[0], N = wr.shape[1], rows = a.numel() / Kd;
+    Tensor w = get_weight(oi, 1, false, false, true);
+    Tensor bb, rr;
+    if (bias) { bb = *bias; if (bb.type != DType::f32) bb = convert(bb, DType::f32); }
+    if (residual) { rr = to_plain(*residual); if (rr.type != DType::f32) rr = convert(rr, DType::f32); }
+    std::vector<int64_t> os = a.shape; os.back() = N;
+    Tensor y = make(DType::f32, os);
+    Tensor planes = make(DType::f16, { 3 * rows * Kd });     // the bf16 planes of a (6 bytes per element)
+    const int rc = osb_tc_gemm_f32x_u8w(a.data(), w.data(), N, y.mdata(), bias ? bb.data() : nullptr, residual ? rr.data() : nullptr, rows, N, Kd, w.scale,
+                                        w.zero_point, planes.mdata(), st);
+    if (rc == (int)cudaErrorNotSupported) return false;
+    ck(rc, "osb_tc_gemm_f32x_u8w");
+    push(out_oi, 0, y);
+    return true;
+}
+
+// out [rows, N] = x . W of the attention projection at op oi, its uint8 weight read as stored (mha_u8w); refused, the fp32 GEMM on its
+// fp32 copy, as before
+void Engine::Impl::u8w_project(size_t oi, const Tensor& x, int64_t rows, Tensor& out)
+{
+    const TensorRef& wr = E.m_ops[oi].in[1];
+    const int64_t Kd = wr.shape[0], N = wr.shape[1];
+    if (osb_tc_gemm_f32x_u8w_ok(rows, N, Kd, N, wr.zero_point)) {
+        Tensor w = get_weight(oi, 1, false, false, true);
+        Tensor planes = make(DType::f16, { 3 * rows * Kd });
+        const int rc = osb_tc_gemm_f32x_u8w(x.data(), w.data(), N, out.mdata(), nullptr, nullptr, rows, N, Kd, w.scale, w.zero_point, planes.mdata(), st);
+        if (rc != (int)cudaErrorNotSupported) { ck(rc, "osb_tc_gemm_f32x_u8w"); return; }
+    }
+    Tensor w = in(oi, 1);
+    if (w.type != x.type) w = convert(w, x.type);
+    ck(osb_gemm(x.data(), w.data(), out.mdata(), nullptr, nullptr, 1, rows, N, Kd, 0, 0, 0, 0, K(x.type), E.gemm_impl, st), "osb_gemm(projection)");
+}
+
 // Gemm (src/onnxstream.cpp:4300-4375)
 void Engine::Impl::op_gemm(size_t oi)
 {
@@ -1025,6 +1101,10 @@ void Engine::Impl::op_gemm(size_t oi)
     if (a.shape.size() == 2 && f16w_gemm(op, a) && op.in[2].present) {
         Tensor c = in(oi, 2);
         if (c.numel() == op.in[1].shape[1] && f16w_gemm_run(oi, a, &c, nullptr, oi)) return;
+    }
+    if (a.shape.size() == 2 && u8w_gemm(op, a) && op.in[2].present) {
+        Tensor c = in(oi, 2);
+        if (c.numel() == op.in[1].shape[1] && u8w_gemm_run(oi, a, &c, nullptr, oi)) return;
     }
     Tensor b = in(oi, 1), c = in(oi, 2);
     if (a.shape.size() != 2 || b.shape.size() != 2) throw std::runtime_error("XnnPack::matrix_multiply_fp32: not implemented (shape of inputs).");
@@ -1929,6 +2009,20 @@ void Engine::Impl::fused_attention(const Step& s)
 void Engine::Impl::mha_project(size_t i, const Tensor& x, const Tensor* xq, Tensor* ql, Tensor& kl, Tensor& vl, int64_t Tka)
 {
     Tensor xk = to_plain(in(i + 4, 0)), xv = to_plain(in(i + 9, 0));
+    if (mha_u8w(i, x.type)) {
+        // W8A32: each projection on its uint8 weight as stored, one launch each
+        if (xk.type != x.type) xk = convert(xk, x.type);
+        if (xv.type != x.type) xv = convert(xv, x.type);
+        const int64_t T = E.m_ops[i + 3].out[0].shape[1], Tk = E.m_ops[i + 8].out[0].shape[2], C = kl.shape[1];
+        if (Tka != Tk) {   // zero pad rows, as below
+            ck(cudaMemsetAsync((char*)kl.mdata() + Tk * C * 4, 0, (Tka - Tk) * C * 4, st), "cudaMemsetAsync");
+            ck(cudaMemsetAsync((char*)vl.mdata() + Tk * C * 4, 0, (Tka - Tk) * C * 4, st), "cudaMemsetAsync");
+        }
+        if (ql) u8w_project(i, *xq, T, *ql);
+        u8w_project(i + 4, xk, Tk, kl);
+        u8w_project(i + 9, xv, Tk, vl);
+        return;
+    }
     Tensor wq = in(i, 1), wk = in(i + 4, 1), wv = in(i + 9, 1);
     const DType ty = x.type;
     if (xk.type != ty) xk = convert(xk, ty);
@@ -1991,7 +2085,15 @@ void Engine::Impl::fused_mha(const Step& s)
     size_t i = s.first;
     const OpDef& op = E.m_ops[i];
     Tensor x = to_plain(in(i, 0)), xk = to_plain(in(i + 4, 0)), xv = to_plain(in(i + 9, 0));
-    Tensor wq = in(i, 1), wk = in(i + 4, 1), wv = in(i + 9, 1);
+    // W8A32: the projections read their uint8 weights as stored (mha_project), so no fp32 copy is fetched here
+    const bool u8p = mha_u8w(i, x.type);
+    Tensor wq, wk, wv;
+    if (u8p) {     // shape-only stand-ins of the activation type, for the checks below; no data is fetched or converted
+        for (Tensor* w : { &wq, &wk, &wv }) w->type = DType::f32;
+        wq.shape = op.in[1].shape; wk.shape = E.m_ops[i + 4].in[1].shape; wv.shape = E.m_ops[i + 9].in[1].shape;
+    } else {
+        wq = in(i, 1); wk = in(i + 4, 1); wv = in(i + 9, 1);
+    }
     for (size_t k : { (size_t)1, (size_t)3, (size_t)5, (size_t)7, (size_t)10, (size_t)12, (size_t)17, (size_t)19 }) (void)in(i + k, 1);   // shape constants: validated statically
     DType ty = x.type;
     if (ty != DType::f16 && ty != DType::f32) fail(op, "wrong data type of input 0.");
@@ -2018,7 +2120,8 @@ void Engine::Impl::fused_mha(const Step& s)
         kl = pre->second.kl; vl = pre->second.vl;
         ck(cudaStreamWaitEvent(st, pre->second.ev, 0), "cudaStreamWaitEvent(main, side K/V)");
         mha_kv.erase(pre);
-        ck(osb_gemm(x.data(), wq.data(), ql.mdata(), nullptr, nullptr, 1, T, C, x.shape[2], 0, 0, 0, 0, K(ty), E.gemm_impl, st), "osb_gemm(q)");
+        if (u8p) u8w_project(i, x, T, ql);
+        else ck(osb_gemm(x.data(), wq.data(), ql.mdata(), nullptr, nullptr, 1, T, C, x.shape[2], 0, 0, 0, 0, K(ty), E.gemm_impl, st), "osb_gemm(q)");
     } else {
         kl = make(ty, { Tka, C }); vl = make(ty, { Tka, C });
         mha_project(i, x, &x, &ql, kl, vl, Tka);

@@ -86,6 +86,8 @@ struct TcParams {
     long long ldc;               // elements between output rows (== N for a dense C)
     int bm, bn;                  // the tile shape the launch runs (the kernel's template arguments; kept for the launch profile)
     int geglu;                   // GEGLU epilogue (osb_tc_gemm_geglu): B is [K, 2 N], C [M, N] = value * gelu(gate)
+    float wscale;                // uint8 weight (tc_gemm_u8w_kernel): per-tensor scale and zero point
+    int wzero;
 };
 
 using namespace tcptx;
@@ -521,6 +523,16 @@ __global__ void splitk_reduce_f32_kernel(const float* __restrict__ ws, float* __
 // weights in B).  B is the OHWI fp16 blob [Cout][kh kw Cin] as stored, K-major, as the fp16 conv reads it.  An unsplit launch stores fp32
 // from the registers (acc + bias[n] + residual, the reduce kernel's order), so the output is not bounded by the workspace; a split
 // launch writes its partials to the workspace for splitk_reduce_f32_kernel.  Ragged Cout stores are guarded by column.
+//
+// U8 (tc_gemm_u8w_kernel: osb_tc_gemm_f32x_u8w, osb_tc_conv_f32x_u8w): the weight is a uint8 blob with a per-tensor scale s and zero
+// point z.  q - z is an integer of at most 255 in magnitude, exact as one bf16, and each product of a bf16 part of x with it has at most 16
+// significant bits, so x (q - z) = h (q - z) + m (q - z) + l (q - z) exactly: three products per stage, (l, q), (m, q), (h, q), small ones
+// first.  Warp 0 lands the uint8 block as stored (GEMM: [64 k][128 n] of the [K][N] blob; CONV: [128 n][64 k] of the OHWI blob, both
+// unswizzled) in a buffer of its own; warps 1-3 write bf16(q - z) into the 128B-swizzled layout the consumers read (MN-major 64-column atoms
+// for the GEMM, K-major rows for the conv) -- GEMM rows past K as 0, since A reads the next plane there.  s is applied once, in fp32, in the
+// epilogue: unsplit, acc s + bias + residual is stored from the registers (GEMM and conv alike, so no output bound from the workspace);
+// split, acc s goes to the workspace for the unchanged splitk_reduce_f32_kernel.  A stage is 48 KB of A planes + 16 KB of bf16 B + 8 KB
+// landing, 3 stages.
 namespace f16w {
 constexpr int A_PLANE_BYTES = BLOCK_M * BLOCK_K * 2;            // 16 KB
 constexpr int A_BYTES = 3 * A_PLANE_BYTES;
@@ -529,6 +541,26 @@ constexpr int B_BYTES = 2 * B_PART_BYTES;
 constexpr int STAGES = 2;
 constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
 constexpr int SPLIT_THREADS = 96;
+// U8: the bf16 (q - z) block, then the uint8 block as it lands
+constexpr int U8_LAND_BYTES = BLOCK_N * BLOCK_K;                // 8 KB
+constexpr int U8_B_BYTES = B_PART_BYTES + U8_LAND_BYTES;
+constexpr int U8_STAGES = 3;
+constexpr int U8_SMEM_BYTES = U8_STAGES * (A_BYTES + U8_B_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
+static_assert(U8_SMEM_BYTES <= 227 * 1024 && U8_B_BYTES % 1024 == 0, "three uint8 stages fit, every bf16 B block on a swizzle boundary");
+}
+
+// 8 uint8 weights (two words) -> 8 bf16 (q - z), exact: 2^23 + q is a float whose low byte is q, and subtracting 2^23 + z (fz) leaves q - z
+__device__ __forceinline__ uint4 u8x8_bf16_minus_zero(uint2 v, float fz)
+{
+    uint32_t o[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const uint32_t w = i < 2 ? v.x : v.y, b = 2 * (i & 1);
+        const float f0 = __uint_as_float(__byte_perm(w, 0x4Bu, 0x4550u + b)) - fz, f1 = __uint_as_float(__byte_perm(w, 0x4Bu, 0x4551u + b)) - fz;
+        const __nv_bfloat162 h = __floats2bfloat162_rn(f0, f1);
+        o[i] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+    return make_uint4(o[0], o[1], o[2], o[3]);
 }
 
 // two fp16 values (one 32-bit word) -> their bf16 hi and lo parts
@@ -543,17 +575,19 @@ __device__ __forceinline__ void f16x2_bf16_parts(uint32_t v, uint32_t& hi, uint3
 }
 
 // p: M, N, K, m_tiles, n_tiles, k_blocks_per_tap (= ceil(K / 64)), split_k, ws; CONV also the conv geometry (K = Cin, M = Ho Wo, taps,
-// kw, pads, stride, bw x bh boxes, tiles_x) and, unsplit, C / bias / residual as fp32
-template <bool CONV>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const TcParams p)
+// kw, pads, stride, bw x bh boxes, tiles_x) and, unsplit, C / bias / residual as fp32; U8 also wscale, wzero and, unsplit, C / bias /
+// residual as fp32 in the GEMM mode too.  The body of tc_gemm_f16w_kernel (U8 = false) and tc_gemm_u8w_kernel (U8 = true); map_a, map_b and
+// p are the kernel's own parameters.
+template <bool CONV, bool U8>
+__device__ __forceinline__ void f16w_u8w_body(const CUtensorMap& map_a, const CUtensorMap& map_b, const TcParams& p)
 {
     using namespace f16w;
+    constexpr int STAGES = U8 ? U8_STAGES : f16w::STAGES, B_BYTES = U8 ? U8_B_BYTES : f16w::B_BYTES;
     osb_pdl_trigger_entry();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* smem_a = smem;                             // [STAGES][3 planes][128 rows][64]
-    uint8_t* smem_b = smem + STAGES * A_BYTES;          // [STAGES][hi, lo][2 atoms][64 k][64]
+    uint8_t* smem_b = smem + STAGES * A_BYTES;          // [STAGES][hi, lo][2 atoms][64 k][64]; U8: [STAGES][q - z, landed uint8]
     uint64_t* bars = (uint64_t*)(smem + STAGES * (A_BYTES + B_BYTES));
     uint64_t* full = bars;
     uint64_t* empty = bars + STAGES;
@@ -593,19 +627,23 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
             for (int kb = kb_lo; kb < kb_hi; kb++) {
                 mbar_wait(&empty[stage], phase ^ 1);
                 if (elect_one()) {
-                    mbar_expect_tx(&landed[stage], A_BYTES + B_PART_BYTES);
+                    mbar_expect_tx(&landed[stage], A_BYTES + (U8 ? U8_LAND_BYTES : B_PART_BYTES));
                     const uint32_t sa = sa0 + stage * A_BYTES, sb = sb0 + stage * B_BYTES;
                     if constexpr (CONV) {
                         const int kc = kcb * BLOCK_K;
 #pragma unroll
                         for (int pl = 0; pl < 3; pl++) tma_load_4d_s(sa + pl * A_PLANE_BYTES, &map_a, &landed[stage], kc, pl, ax + kx, ay + ky);
-                        tma_load_3d_s(sb, &map_b, &landed[stage], tap * p.K + kc, n0, 0);
+                        tma_load_3d_s(U8 ? sb + B_PART_BYTES : sb, &map_b, &landed[stage], tap * p.K + kc, n0, 0);
                     } else {
                         const int kc = kb * BLOCK_K;
 #pragma unroll
                         for (int pl = 0; pl < 3; pl++) tma_load_3d_s(sa + pl * A_PLANE_BYTES, &map_a, &landed[stage], pl * p.K + kc, m0, 0);
+                        if constexpr (U8) {
+                            tma_load_3d_s(sb + B_PART_BYTES, &map_b, &landed[stage], n0, kc, 0);     // one [64 k][128 n] uint8 box
+                        } else {
 #pragma unroll
-                        for (int at = 0; at < 2; at++) tma_load_3d_s(sb + at * 8192, &map_b, &landed[stage], n0 + 64 * at, kc, 0);
+                            for (int at = 0; at < 2; at++) tma_load_3d_s(sb + at * 8192, &map_b, &landed[stage], n0 + 64 * at, kc, 0);
+                        }
                     }
                 }
                 __syncwarp();
@@ -616,6 +654,40 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
             }
         }
         osb_pdl_trigger_late();
+    } else if (U8 && warp < 4) {
+        // ===================== B converters: uint8 q -> bf16 (q - z) in the swizzled layout, once per raw block =====================
+        // 8 landed bytes per thread -> one 16-byte chunk of a 128-byte swizzle row: chunk c of row r sits at chunk c ^ (r & 7)
+        const int t = (int)threadIdx.x - 32;
+        const float fz = 8388608.f + (float)p.wzero;
+        int stage = 0; uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+            const int sp = tile % p.split_k;
+            const int kb_lo = sp * kb_per_split, kb_hi = min(kb_lo + kb_per_split, kbk);
+            for (int kb = kb_lo; kb < kb_hi; kb++) {
+                mbar_wait(&landed[stage], phase);
+                uint8_t* bq = smem_b + stage * B_BYTES;
+                const uint2* land = reinterpret_cast<const uint2*>(bq + B_PART_BYTES);
+                const int k_valid = CONV ? BLOCK_K : p.K - kb * BLOCK_K;     // GEMM: the block's rows inside K
+#pragma unroll 4
+                for (int g = t; g < U8_LAND_BYTES / 8; g += SPLIT_THREADS) {
+                    uint4 o = u8x8_bf16_minus_zero(land[g], fz);
+                    int off;
+                    if constexpr (CONV) {
+                        const int n = g >> 3, c = g & 7;            // landed row n: 64 k = 8 chunks
+                        off = n * 128 + ((c ^ (n & 7)) << 4);
+                    } else {
+                        const int k = g >> 4, c = g & 15;           // landed row k: 128 n = 16 chunks, two 64-column atoms
+                        off = (c >> 3) * 8192 + k * 128 + (((c & 7) ^ (k & 7)) << 4);
+                        if (k >= k_valid) o = make_uint4(0u, 0u, 0u, 0u);
+                    }
+                    *reinterpret_cast<uint4*>(bq + off) = o;
+                }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor cores
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&full[stage]);
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+        }
     } else if (warp < 4) {
         // ===================== B splitters: fp16 -> hi (in place) and lo, once per raw block =====================
         const int t = (int)threadIdx.x - 32;
@@ -647,7 +719,7 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
             }
         }
     } else {
-        // ===================== consumers: 5 products per stage, fp32 partials out =====================
+        // ===================== consumers: 5 products per stage (U8: 3), fp32 partials out =====================
         const int wg = (warp >> 2) - 1;
         const uint64_t adesc0 = make_smem_desc(smem_u32(smem_a) + 64 * wg * 128, 16, 1024);
         // B: MN-major (GEMM: [K][N] weight, two 64-column atoms) or K-major (CONV: 128 OHWI rows of 64 k)
@@ -668,11 +740,11 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
             for (int kb = kb_lo; kb < kb_hi; kb++) {
                 mbar_wait(&full[stage], phase);
                 const uint64_t a = adesc0 + (uint64_t)(stage * (A_BYTES >> 4)), b = bdesc0 + (uint64_t)(stage * (B_BYTES >> 4));
-                // (A plane, B part): (h, hi), (h, lo), (m, hi), (l, hi), (m, lo)
-                const uint64_t ad[5] = { a, a, a + AP, a + 2 * AP, a + AP }, bd[5] = { b, b + BP, b, b, b + BP };
+                // (A plane, B part): (h, hi), (h, lo), (m, hi), (l, hi), (m, lo); U8: (l, q), (m, q), (h, q)
+                const uint64_t ad[5] = { U8 ? a + 2 * AP : a, U8 ? a + AP : a, U8 ? a : a + AP, a + 2 * AP, a + AP }, bd[5] = { b, U8 ? b : b + BP, b, b, b + BP };
                 wgmma_fence();
 #pragma unroll
-                for (int x = 0; x < 5; x++) {
+                for (int x = 0; x < (U8 ? 3 : 5); x++) {
 #pragma unroll
                     for (int k = 0; k < BLOCK_K / WG_K; k++)
                         wgmma_ss<128, CONV ? 0 : 1, true>(acc, ad[x] + (uint64_t)(k * ((WG_K * 2) >> 4)), bd[x] + (uint64_t)(k * b_kstep), 1u);
@@ -684,17 +756,24 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
             }
             wgmma_wait<0>();
             mbar_arrive(&empty[prev]);
-            if constexpr (CONV) {
-                // the tile's rows are a bw x bh box of output pixels
-                const int mt = r % p.m_tiles, ty = (mt / p.tiles_x) * p.bh, tx = (mt % p.tiles_x) * p.bw;
+            if constexpr (CONV || U8) {
+                // CONV: the tile's rows are a bw x bh box of output pixels
+                const int mt = r % p.m_tiles, ty = CONV ? (mt / p.tiles_x) * p.bh : 0, tx = CONV ? (mt % p.tiles_x) * p.bw : 0;
                 const float* bias = reinterpret_cast<const float*>(p.bias);
                 const float* res = reinterpret_cast<const float*>(p.residual);
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
-                    const int rt = r_lo + 8 * h, y = ty + rt / p.bw, x = tx + rt % p.bw;
-                    if (y >= p.Ho || x >= p.Wo) continue;
-                    const long long row = (long long)y * p.Wo + x;
-                    // split: raw partials -> ws[sp][M][N]; unsplit: acc + bias + residual -> C, fp32
+                    const int rt = r_lo + 8 * h;
+                    long long row;
+                    if constexpr (CONV) {
+                        const int y = ty + rt / p.bw, x = tx + rt % p.bw;
+                        if (y >= p.Ho || x >= p.Wo) continue;
+                        row = (long long)y * p.Wo + x;
+                    } else {
+                        if (m0 + rt >= p.M) continue;
+                        row = m0 + rt;
+                    }
+                    // split: raw partials (U8: times s) -> ws[sp][M][N]; unsplit: acc (U8: times s) + bias + residual -> C, fp32
                     float* out = p.split_k > 1 ? p.ws + ((long long)sp * p.M + row) * p.N : reinterpret_cast<float*>(p.C) + row * p.N;
                     const float* rrow = p.split_k > 1 || !res ? nullptr : res + row * p.N;
                     const float* b = p.split_k > 1 ? nullptr : bias;
@@ -703,6 +782,7 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
                         const int n = n0 + 8 * j + cq;
                         const bool ok0 = n < p.N, ok1 = n + 1 < p.N;
                         float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+                        if constexpr (U8) { f0 = __fmul_rn(f0, p.wscale); f1 = __fmul_rn(f1, p.wscale); }   // rounded before the bias, as a split launch does
                         if (b) { if (ok0) f0 += b[n]; if (ok1) f1 += b[n + 1]; }
                         if (rrow) {
                             if (ok1 && pair_ok) { const float2 rv = *reinterpret_cast<const float2*>(rrow + n); f0 += rv.x; f1 += rv.y; }
@@ -732,6 +812,20 @@ tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_cons
     }
 }
 
+template <bool CONV>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+tc_gemm_f16w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const TcParams p)
+{
+    f16w_u8w_body<CONV, false>(map_a, map_b, p);
+}
+
+template <bool CONV>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+tc_gemm_u8w_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const TcParams p)
+{
+    f16w_u8w_body<CONV, true>(map_a, map_b, p);
+}
+
 #include "gemm_i8.cuh"
 
 // ---- host side -------------------------------------------------------------------------------------------------
@@ -740,10 +834,10 @@ constexpr size_t WS_MAX = OSB_WS_SPLITK_BYTES;   // fixed-capacity per-stream wo
 int num_sms();
 
 // The previous rule, kept selectable (osb_tc_set_tile(-1, 0, 0)) for A/B runs: 128 x 128 tiles, split K when there are fewer than 100 tiles
-// and at least 32 k-blocks, fill the SMs, keep >= 2 k-blocks per split, stay inside the workspace
-int old_split(int tiles, int k_blocks, size_t out_elems)
+// and at least 32 (min_k_blocks) k-blocks, fill the SMs, keep >= 2 k-blocks per split, stay inside the workspace
+int old_split(int tiles, int k_blocks, size_t out_elems, int min_k_blocks = 32)
 {
-    if (tiles >= 100 || k_blocks < 32) return 1;
+    if (tiles >= 100 || k_blocks < min_k_blocks) return 1;
     int split = std::min(num_sms() / tiles, k_blocks / 2);
     while (split > 1 && (size_t)split * out_elems * 4 > WS_MAX) split--;
     if (split <= 1) return 1;
@@ -1531,4 +1625,122 @@ extern "C" int osb_tc_conv_f32x_f16w(const void* x, const void* w, const void* b
     osb_launch((splitk_reduce_f32_kernel), (int)std::min<long long>((total + 255) / 256, num_sms() * 8), 256, 0, st, (const float*)p.ws, (float*)y,
                (const float*)bias, (const float*)residual, (long long)M, (int)Cout, split);
     return launched();
+}
+
+// ---- fp32 GEMM and conv on a uint8 weight read in place ---------------------------------------------------------------------------------
+// The split rule of the fp16-weight launches (old_split: fewer than 100 tiles fill the SMs, >= 2 k-blocks per split) over the raw k-blocks,
+// from 10 of them instead of 32: a k-block here is three products deep.  SDXL's few-tile launches of 10-31 k-blocks (the 1x1 skip convs at
+// 16 x 16 and 32 x 32, its 256-row GEMMs) ran up to 1.6x slower than the expanded route unsplit and 1.1-1.5x faster split (H100, DESIGN.md
+// section 5).  osb_tc_set_tile's forced split, clamped so that no split is empty; a split runs only where its partials fit the workspace
+// (unsplit, the kernel stores the output).
+static int u8w_split(const TileProblem& q, int k_blocks, size_t out_elems)
+{
+    int split = old_split(problem_m_tiles(q, BLOCK_M) * ((q.N + BLOCK_N - 1) / BLOCK_N), k_blocks, out_elems, 10);
+    if (g_tile_split > 0) {
+        split = std::min(g_tile_split, k_blocks);
+        if (split > 1) { const int kb_per = (k_blocks + split - 1) / split; split = (k_blocks + kb_per - 1) / kb_per; }
+    }
+    if ((size_t)split * out_elems * 4 > WS_MAX) split = 1;
+    return split;
+}
+
+// the uint8 launch: the split of the activation into `planes` (done by the caller), tc_gemm_u8w_kernel, and the fp32 reduce
+// when the launch splits K
+template <bool CONV>
+static int u8w_launch(const CUtensorMap& ma, const CUtensorMap& mb, TcParams& p, int split, const void* y, const void* bias, const void* residual, cudaStream_t st)
+{
+    static const cudaError_t attr = cudaFuncSetAttribute(tc_gemm_u8w_kernel<CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, f16w::U8_SMEM_BYTES);
+    if (attr != cudaSuccess) return (int)attr;
+    OsbWorkspace* wsp = split > 1 ? osb_workspace(st, OSB_WS_SPLITK) : nullptr;
+    if (!wsp) split = 1;
+    p.split_k = split;
+    p.ws = wsp ? wsp->splitk : nullptr;
+    p.C = (__half*)y; p.bias = (const __half*)bias; p.residual = (const __half*)residual; p.ldc = p.N;   // fp32 (see the kernel)
+    const int grid = (int)std::min<int64_t>((int64_t)p.m_tiles * p.n_tiles * split, num_sms());
+    osb_launch((tc_gemm_u8w_kernel<CONV>), grid, NUM_THREADS, (size_t)f16w::U8_SMEM_BYTES, st, ma, mb, p);
+    int e = launched(1);
+    if (e || split == 1) return e;
+    const long long total = (long long)p.M * p.N;
+    osb_launch((splitk_reduce_f32_kernel), (int)std::min<long long>((total + 255) / 256, num_sms() * 8), 256, 0, st, (const float*)p.ws, (float*)y,
+               (const float*)bias, (const float*)residual, (long long)p.M, p.N, split);
+    return launched();
+}
+
+extern "C" int osb_tc_gemm_f32x_u8w_ok(int64_t M, int64_t N, int64_t K, int64_t ldb, int zero_point)
+{
+    return f32_tc_on() && M >= 1 && N >= 1 && K >= 8 && K % 8 == 0 && ldb % 16 == 0 && ldb >= N && M <= (1 << 30) && ldb <= (1 << 30) &&
+           3 * K <= (1 << 30) && zero_point >= 0 && zero_point <= 255 && get_encode() != nullptr ? 1 : 0;
+}
+
+// C [M, N] fp32 = A [M, K] fp32 . ((B [K, N] uint8, rows ldb apart) - zero_point) scale + bias [N] + residual [M, N] (fp32, either may be null)
+extern "C" int osb_tc_gemm_f32x_u8w(const void* A, const void* B, int64_t ldb, void* C, const void* bias, const void* residual, int64_t M, int64_t N,
+                                    int64_t K, float scale, int zero_point, void* planes, void* stream)
+{
+    if (!osb_tc_gemm_f32x_u8w_ok(M, N, K, ldb, zero_point) || !aligned16(A) || !aligned16(B) || !aligned16(planes) || ((uintptr_t)C & 7) ||
+        ((uintptr_t)bias & 3) || ((uintptr_t)residual & 7))
+        return (int)cudaErrorNotSupported;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t K3 = 3 * K;
+    const int kbk = (int)((K + BLOCK_K - 1) / BLOCK_K);
+    CUtensorMap ma, mb;
+    int sw = 0;
+    // A: the planes [M][3][K] as one [M, 3 K] map (a chunk past K reads the next plane, against B rows the converters zero)
+    if (!make_map_rb(&ma, planes, (uint64_t)K3, (uint64_t)M, 1, (uint64_t)K3 * 2, (uint64_t)(M * K3) * 2, BLOCK_K, BLOCK_M, &sw)) return (int)cudaErrorNotSupported;
+    // B: the [K][N] uint8 blob, one unswizzled [64 k][128 n] box per k-block
+    if (!make_map(&mb, B, (uint64_t)N, (uint64_t)K, 1, (uint64_t)ldb, (uint64_t)(K * ldb), BLOCK_N, BLOCK_K, 1, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8,
+                  CU_TENSOR_MAP_SWIZZLE_NONE))
+        return (int)cudaErrorNotSupported;
+    TcParams p{};
+    p.M = (int)M; p.N = (int)N; p.K = (int)K; p.batch = 1;
+    p.bm = BLOCK_M; p.bn = BLOCK_N;
+    p.m_tiles = (int)((M + BLOCK_M - 1) / BLOCK_M); p.n_tiles = (int)((N + BLOCK_N - 1) / BLOCK_N);
+    p.k_blocks_per_tap = kbk;
+    p.wscale = scale; p.wzero = zero_point;
+    const int split = u8w_split(TileProblem{ (int)M, (int)N, 0, 0, 0, 1, kbk, 0, true, true }, kbk, (size_t)M * N);
+    int e = osb_f32x_split_rows((const float*)A, (__nv_bfloat16*)planes, M, K, st);
+    if (e) return e;
+    return u8w_launch<false>(ma, mb, p, split, C, bias, residual, st);
+}
+
+extern "C" int osb_tc_conv_f32x_u8w_ok(int64_t H, int64_t W, int64_t Cin, int64_t Cout, int kh, int kw, int stride, int64_t Ho, int64_t Wo, int zero_point)
+{
+    return osb_tc_conv_f32x_f16w_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo) && ((int64_t)kh * kw * Cin) % 16 == 0 && zero_point >= 0 && zero_point <= 255 ? 1 : 0;
+}
+
+// y [Ho, Wo, Cout] fp32 = conv(x [H, W, Cin] fp32, (w [Cout][kh][kw][Cin] uint8 - zero_point) scale) + bias [Cout] + residual [Ho, Wo, Cout]
+extern "C" int osb_tc_conv_f32x_u8w(const void* x, const void* w, const void* bias, const void* residual, void* y, int64_t H, int64_t W, int64_t Cin,
+                                    int64_t Cout, int kh, int kw, int stride, int pad_top, int pad_left, int64_t Ho, int64_t Wo, float scale, int zero_point,
+                                    void* planes, void* stream)
+{
+    if (!osb_tc_conv_f32x_u8w_ok(H, W, Cin, Cout, kh, kw, stride, Ho, Wo, zero_point) || !aligned16(x) || !aligned16(w) || !aligned16(planes) ||
+        ((uintptr_t)y & 7) || ((uintptr_t)bias & 3) || ((uintptr_t)residual & 7))
+        return (int)cudaErrorNotSupported;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int kbpt = (int)((Cin + BLOCK_K - 1) / BLOCK_K), k_blocks = kh * kw * kbpt;
+    const int64_t M = Ho * Wo, Ktot = (int64_t)kh * kw * Cin;
+    const uint32_t bw = (uint32_t)conv_box_w(BLOCK_M, (int)Wo), bh = BLOCK_M / bw;
+    CUtensorMap ma, mb;
+    // A: the planes [H][W][3][Cin] as (Cin, plane, W, H), as in osb_tc_conv_f32x_f16w
+    if (!make_map_4d(&ma, planes, (uint64_t)Cin, 3, (uint64_t)W, (uint64_t)H, (uint64_t)Cin * 2, (uint64_t)Cin * 6, (uint64_t)W * Cin * 6, BLOCK_K, 1,
+                     bw * stride, bh * stride, (uint32_t)stride))
+        return (int)cudaErrorNotSupported;
+    // B: the OHWI uint8 blob [Cout][kh kw Cin], one unswizzled [128 n][64 k] box per k-block
+    if (!make_map(&mb, w, (uint64_t)Ktot, (uint64_t)Cout, 1, (uint64_t)Ktot, (uint64_t)(Ktot * Cout), BLOCK_K, BLOCK_N, 1, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8,
+                  CU_TENSOR_MAP_SWIZZLE_NONE))
+        return (int)cudaErrorNotSupported;
+    TcParams p{};
+    p.M = (int)M; p.N = (int)Cout; p.K = (int)Cin; p.batch = 1;
+    p.bm = BLOCK_M; p.bn = BLOCK_N;
+    p.tiles_x = (int)((Wo + bw - 1) / bw);
+    p.m_tiles = p.tiles_x * (int)((Ho + bh - 1) / bh);
+    p.n_tiles = (int)((Cout + BLOCK_N - 1) / BLOCK_N);
+    p.b_kmajor = 1;
+    p.taps = kh * kw; p.kw = kw; p.pad_top = pad_top; p.pad_left = pad_left; p.Wo = (int)Wo; p.Ho = (int)Ho; p.bw = (int)bw; p.bh = (int)bh;
+    p.k_blocks_per_tap = kbpt;
+    p.stride = stride;
+    p.wscale = scale; p.wzero = zero_point;
+    const int split = u8w_split(TileProblem{ (int)M, (int)Cout, (int)Ho, (int)Wo, 1, 1, k_blocks, 1, true, true }, k_blocks, (size_t)M * Cout);
+    int e = osb_f32x_split_rows((const float*)x, (__nv_bfloat16*)planes, H * W, Cin, st);
+    if (e) return e;
+    return u8w_launch<true>(ma, mb, p, split, y, bias, residual, st);
 }

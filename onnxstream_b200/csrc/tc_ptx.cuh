@@ -25,9 +25,10 @@ inline PFN_cuTensorMapEncodeTiled_v12000 get_encode()
     return fn;
 }
 
-// rank-3 fp16 tensor map with 128B swizzle; dims/strides innermost first
+// rank-3 fp16 tensor map with 128B swizzle (or `swizzle`); dims/strides innermost first
 inline bool make_map(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1_bytes, uint64_t s2_bytes,
-                     uint32_t b0, uint32_t b1, uint32_t b2, uint32_t traversal_stride = 1, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16)
+                     uint32_t b0, uint32_t b1, uint32_t b2, uint32_t traversal_stride = 1, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                     CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B)
 {
     auto enc = get_encode();
     if (!enc) return false;
@@ -36,7 +37,7 @@ inline bool make_map(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d
     cuuint32_t box[3] = { b0, b1, b2 };
     cuuint32_t estr[3] = { 1, traversal_stride, traversal_stride };   // strided conv: every s-th pixel of the box span
     CUresult r = enc(map, dtype, 3, const_cast<void*>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS;
 }
