@@ -362,7 +362,7 @@ def _nodes(d):
 
 
 def _routed(node):
-    """The engine's rule (engine_run.cpp: u8w_weight, u8w_gemm, mha_u8w, op_conv): a Conv the kernel takes, or a MatMul / Gemm with a 2-D
+    """The engine's rule (engine_run.cpp: weight_route, mha_stored): a Conv the kernel takes, or a MatMul / Gemm with a 2-D
     weight and more than 2 rows."""
     op, ws, xs, zp = node
     if op == "Conv":
