@@ -635,6 +635,51 @@ static std::vector<int64_t> contiguous_strides(const std::vector<int64_t>& shape
     return s;
 }
 
+// numpy broadcasting of host-evaluated operands (Where, the compare ops): `out` is the broadcast shape of the operands' shapes (empty
+// `ok` when they do not broadcast); for_each(f) calls f(i, off) for every output element i in order, off[k] being operand k's flat
+// source index (the index arithmetic of Expand), advanced like an odometer: no per-element division, no index buffer
+struct Broadcast {
+    std::vector<int64_t> out;
+    std::vector<std::vector<int64_t>> strides;   // per operand, per output dimension; 0 where the operand broadcasts
+    bool ok = true;
+    explicit Broadcast(const std::vector<std::vector<int64_t>>& shapes)
+    {
+        size_t nd = 0;
+        for (auto& s : shapes) nd = std::max(nd, s.size());
+        out.assign(nd, 1);
+        std::vector<std::vector<int64_t>> padded;
+        for (auto& s : shapes) {
+            std::vector<int64_t> p(nd - s.size(), 1);
+            p.insert(p.end(), s.begin(), s.end());
+            for (size_t d = 0; d < nd; d++) {
+                if (p[d] != out[d] && p[d] != 1 && out[d] != 1) ok = false;
+                else if (p[d] != 1) out[d] = p[d];
+            }
+            padded.push_back(std::move(p));
+        }
+        for (auto& p : padded) {
+            auto cs = contiguous_strides(p);
+            for (size_t d = 0; d < nd; d++) if (p[d] == 1) cs[d] = 0;
+            strides.push_back(std::move(cs));
+        }
+    }
+    int64_t numel() const { int64_t n = 1; for (auto d : out) n *= d; return n; }
+    template <class F> void for_each(F f) const
+    {
+        const size_t nd = out.size(), k = strides.size();
+        const int64_t n = numel();
+        std::vector<int64_t> idx(nd, 0), off(k, 0);
+        for (int64_t i = 0; i < n; i++) {
+            f((size_t)i, off.data());
+            for (size_t d = nd; d-- > 0;) {
+                if (++idx[d] < out[d]) { for (size_t j = 0; j < k; j++) off[j] += strides[j][d]; break; }
+                idx[d] = 0;
+                for (size_t j = 0; j < k; j++) off[j] -= strides[j][d] * (out[d] - 1);
+            }
+        }
+    }
+};
+
 static float scalar_of(const Tensor& t, const OpDef& op)
 {
     if (t.host_f32 && !t.host_f32->empty()) return (*t.host_f32)[0];
@@ -1303,7 +1348,16 @@ void Engine::Impl::op_concat(size_t oi)
         push(oi, 0, r);
         return;
     }
-    DType ty = xs[0].type;
+    // uint8 sources (uint8 arithmetic) are copied as bytes only when every non-empty one carries the same scale and zero point.  Otherwise
+    // each is dequantised at its own scale, and push re-quantises the float result by the percentile rule like any float output.
+    size_t first = 0;
+    while (first + 1 < xs.size() && xs[first].numel() == 0) first++;
+    bool mixed_q = false;
+    for (auto& t : xs)
+        if (t.numel() != 0 && (t.type != xs[first].type || (t.type == DType::u8 && (t.scale != xs[first].scale || t.zero_point != xs[first].zero_point))))
+            mixed_q = true;
+    if (mixed_q) for (auto& t : xs) if (t.type == DType::u8) t = dequantize(t, act_dtype());
+    DType ty = xs[first].type;
     bool all_nhwc = true;
     for (auto& t : xs) { if (t.layout != Layout::nhwc) all_nhwc = false; }
     bool nhwc_path = all_nhwc && axis == 1 && rank == 4 && E.keep_nhwc;
@@ -1321,7 +1375,7 @@ void Engine::Impl::op_concat(size_t oi)
             if (xs[e].numel() == 0) { Tensor r = xs[1 - e]; r.shape = os; push(oi, 0, r); return; }
     }
     Tensor y = make(ty, os, nhwc_path ? Layout::nhwc : Layout::plain);
-    y.scale = xs[0].scale; y.zero_point = xs[0].zero_point;
+    y.scale = xs[first].scale; y.zero_point = xs[first].zero_point;
     if (nhwc_path && xs.size() == 2 && stats_want >= 0 && gn_ring && cur_B == 1 && gn_split_enabled() && gn_apply_ok(y, os[1], stats_groups)) {
         // the skip-connection Concat of a UNet up block feeding its GroupNorm: one pass copies and gathers the statistics
         if (osb_concat2_stats(xs[0].data(), xs[1].data(), y.mdata(), K(ty), xs[0].shape[1], xs[1].shape[1], os[2] * os[3], stats_groups, gn_slot_ptr(gn_slot), st) == 0) {
@@ -1680,46 +1734,37 @@ void Engine::Impl::op_misc_host(size_t oi)
     } else if (op.type == "Less" || op.type == "Greater" || op.type == "Equal" || op.type == "And") {
         Tensor a = in(oi, 0), b = in(oi, 1);
         if (a.type != DType::i64 || b.type != DType::i64) fail(op, "only int64 operands are implemented in the engine.");
-        size_t na = a.i64->size(), nb = b.i64->size(), n = std::max(na, nb);
-        if (!(na == nb || na == 1 || nb == 1)) {
-            // outer-product style broadcast [n,1] vs [1,m] / [m]
-            if (a.shape.size() >= 1 && b.shape.size() >= 1 && a.shape.back() == 1 && (int64_t)nb == b.shape.back()) {
-                std::vector<int64_t> v(na * nb);
-                for (size_t i = 0; i < na; i++) for (size_t j = 0; j < nb; j++) {
-                    int64_t x = (*a.i64)[i], y = (*b.i64)[j];
-                    v[i * nb + j] = op.type == "Less" ? x < y : op.type == "Greater" ? x > y : op.type == "Equal" ? x == y : (x && y);
-                }
-                std::vector<int64_t> os = a.shape; os.back() = (int64_t)nb;
-                push(oi, 0, mk_i64(std::move(v), os));
-                return;
-            }
-            fail(op, "broadcast not implemented.");
-        }
-        std::vector<int64_t> v(n);
-        for (size_t i = 0; i < n; i++) {
-            int64_t x = (*a.i64)[na == 1 ? 0 : i], y = (*b.i64)[nb == 1 ? 0 : i];
-            v[i] = op.type == "Less" ? x < y : op.type == "Greater" ? x > y : op.type == "Equal" ? x == y : (x && y);
-        }
-        push(oi, 0, mk_i64(std::move(v), na >= nb ? a.shape : b.shape));
+        if ((size_t)a.numel() != a.i64->size() || (size_t)b.numel() != b.i64->size()) fail(op, "invalid shape of one or more inputs.");
+        const Broadcast bc({ a.shape, b.shape });
+        if (!bc.ok) fail(op, "shapes are not broadcastable.");
+        const int kind = op.type == "Less" ? 0 : op.type == "Greater" ? 1 : op.type == "Equal" ? 2 : 3;
+        std::vector<int64_t> v((size_t)bc.numel());
+        bc.for_each([&](size_t i, const int64_t* off) {
+            const int64_t x = (*a.i64)[off[0]], y = (*b.i64)[off[1]];
+            v[i] = kind == 0 ? x < y : kind == 1 ? x > y : kind == 2 ? x == y : (x && y);
+        });
+        push(oi, 0, mk_i64(std::move(v), bc.out));
     } else if (op.type == "Where") {
         Tensor c = in(oi, 0), x = in(oi, 1), y = in(oi, 2);
         if (c.type != DType::i64) fail(op, "wrong data type of condition.");
+        // condition and branches broadcast against each other (a [1, 1, T, T] causal mask selecting from [1, H, T, T] scores)
+        for (const Tensor* t : { &c, &x, &y })
+            if (t->type == DType::i64 && (size_t)t->numel() != t->i64->size()) fail(op, "invalid shape of one or more inputs.");
+        const Broadcast bc({ c.shape, x.shape, y.shape });
+        if (!bc.ok) fail(op, "shapes are not broadcastable.");
+        const size_t n = (size_t)bc.numel();
         if (x.type == DType::i64 && y.type == DType::i64) {
-            size_t n = c.i64->size(), nx = x.i64->size(), ny = y.i64->size();
-            n = std::max(n, std::max(nx, ny));
             std::vector<int64_t> v(n);
-            for (size_t i = 0; i < n; i++) v[i] = (*c.i64)[c.i64->size() == 1 ? 0 : i] ? (*x.i64)[nx == 1 ? 0 : i] : (*y.i64)[ny == 1 ? 0 : i];
-            push(oi, 0, mk_i64(std::move(v), c.i64->size() == n ? c.shape : (nx == n ? x.shape : y.shape)));
+            bc.for_each([&](size_t i, const int64_t* off) { v[i] = (*c.i64)[off[0]] ? (*x.i64)[off[1]] : (*y.i64)[off[2]]; });
+            push(oi, 0, mk_i64(std::move(v), bc.out));
         } else {
             // float branches: evaluate on the host (masks are tiny), then upload
             auto to_host = [&](Tensor t) { std::vector<float> hv; if (t.type == DType::i64) { hv.resize(t.i64->size()); for (size_t i = 0; i < hv.size(); i++) hv[i] = (float)(*t.i64)[i]; return hv; }
                 Tensor f = convert(to_plain(t), DType::f32); hv.resize((size_t)f.numel()); ck(cudaMemcpyAsync(hv.data(), f.data(), hv.size() * 4, cudaMemcpyDeviceToHost, st), "where D2H"); ck(cudaStreamSynchronize(st), "sync"); return hv; };
             auto hx = to_host(x), hy = to_host(y);
-            size_t n = std::max(c.i64->size(), std::max(hx.size(), hy.size()));
             std::vector<float> hv(n);
-            for (size_t i = 0; i < n; i++) hv[i] = (*c.i64)[c.i64->size() == 1 ? 0 : i] ? hx[hx.size() == 1 ? 0 : i] : hy[hy.size() == 1 ? 0 : i];
-            std::vector<int64_t> os = c.i64->size() == n ? c.shape : (hx.size() == n ? x.shape : y.shape);
-            Tensor f = make(DType::f32, os);
+            bc.for_each([&](size_t i, const int64_t* off) { hv[i] = (*c.i64)[off[0]] ? hx[off[1]] : hy[off[2]]; });
+            Tensor f = make(DType::f32, bc.out);
             ck(cudaMemcpyAsync(f.mdata(), hv.data(), n * 4, cudaMemcpyHostToDevice, st), "where H2D");
             ck(cudaStreamSynchronize(st), "sync");
             push(oi, 0, f);
